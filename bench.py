@@ -11,7 +11,7 @@ on): N=65,536, d=256, ICASSP-2018 refinement sequence, GraphCut Laplacian, eigen
   value : embeddings/s with the embeddings already resident in HBM (CUDA events)
   e2e   : the same metric through the public API -- predict(np.ndarray) -> np.ndarray, the H2D
           copy of the embeddings and the D2H copy of the labels inside the timed region
-  roofline : the dominant kernel (Diffuse, tcgen05 GEMM) against the measured tensor peak
+  roofline : the dominant kernel (Diffuse, wgmma GEMM) against the tensor peak
   cpu_baseline / --impl reference : the NumPy/SciPy/scikit-learn oracle (a restatement of the
           pure-Python reference, which cannot travel to the GPU box) on a bounded sample
 
@@ -57,7 +57,13 @@ def parse():
                   help="--impl reference: also time the CPU path stage by stage at this N, once, "
                        "outside the timed steps (BASELINE.md section 3 planned 16384: ~70 s; the "
                        "default 8192 takes ~15 s; 0 = skip)")
-  return ap.parse_args()
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="predict workload: after the timed steps, write what the last timed step "
+                       "computed (labels, eigenvalues) as DIR/<name>.npy in float64")
+  args = ap.parse_args()
+  if args.dump_outputs and (args.impl != "b200" or args.workload not in ("auto", "predict")):
+    ap.error("--dump-outputs covers the single-process predict workload")
+  return args
 
 
 def workload_name(n, d):
@@ -84,7 +90,7 @@ def make_clusterer():
 
 
 class ClockSampler(threading.Thread):
-  """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+  """nvidia-smi clocks / throttle reasons during the timed region."""
 
   def __init__(self, index):
     super().__init__(daemon=True)
@@ -279,7 +285,7 @@ def run_sharded(args, eng, rank, world, dist):
         "gpu_launches": int(launches),
         "stage_ms_rank0": {k: v / args.steps for k, v in sorted(stages.items())},
         "timeline_ms_rank0_last_step": timeline,
-        "roofline": {"kernel": "k_gemm_tcgen05 (per-peer Diffuse blocks, rank 0)", "bound": "tensor",
+        "roofline": {"kernel": "k_gemm_wgmma (per-peer Diffuse blocks, rank 0)", "bound": "tensor",
                      "achieved": (2.0 * n * n * n / world) / (gemm_ms * 1e-3) / 1e12 if gemm_ms else None,
                      "unit": "TFLOP/s", "traffic": None}}))
   if world > 1:
@@ -291,7 +297,7 @@ def dtype_string(eng, n):
   scheme = {nat.GEMM_SPLIT3: "fp16x3 split (hi*hi + hi*lo + lo*hi)",
             nat.GEMM_SPLIT2: "fp16x2 split ((hi+lo)*hi)",
             nat.GEMM_SINGLE: "fp16 single (hi*hi)"}[eng.diffuse_precision_for(n)]
-  return ("f32 storage; affinity: fp16x3 split tcgen05 MMAs; Diffuse: %s tcgen05 MMAs, f32 "
+  return ("f32 storage; affinity: fp16x3 split wgmma MMAs; Diffuse: %s wgmma MMAs, f32 "
           "two-level accumulate; f64 eigensolve and k-means" % scheme)
 
 
@@ -306,11 +312,11 @@ def roofline_diffuse(eng, n, diffuse_ms, tensor_peak, peak_note, traffic):
   mirrors them (N^3 multiply-adds x 2 / 2 per MMA plane), times the MMAs issued per product.
   SURVEY.md 8(d) quotes 2 N^3 for the full product: reported beside it, not as the fraction."""
   if not diffuse_ms:
-    return {"kernel": "k_gemm_tcgen05 (Diffuse, Y Y^T)", "bound": "tensor", "achieved": None,
+    return {"kernel": "k_gemm_wgmma (Diffuse, Y Y^T)", "bound": "tensor", "achieved": None,
             "peak": tensor_peak, "unit": "TFLOP/s", "frac": None, "traffic": traffic}
   mmas = mma_per_product(eng, n)
   tri = 1.0 * n * n * n / (diffuse_ms * 1e-3) / 1e12          # N^3: the triangle, one MMA per product
-  return {"kernel": "k_gemm_tcgen05 (Diffuse, Y Y^T)", "bound": "tensor",
+  return {"kernel": "k_gemm_wgmma (Diffuse, Y Y^T)", "bound": "tensor",
           "achieved": tri * mmas, "peak": tensor_peak, "unit": "TFLOP/s",
           "frac": tri * mmas / tensor_peak, "traffic": traffic, "peak_source": peak_note,
           "basis": "executed fp16 MMA flop = %d x N^3 (upper-triangle tiles only, %d MMA(s) per "
@@ -351,6 +357,12 @@ def roofline_refinement(eng, n, stages, steps, hbm_peak):
           "moved_GBps": moved * gb / (tot / 1e3) if tot else None,
           "moved_frac": moved * gb / (tot / 1e3) / hbm_peak if tot else None,
           "kernels": how, "peak_GBps": hbm_peak}
+
+
+# NVIDIA's H100 SXM data sheet (700 W card): dense fp16/bf16 tensor rate and HBM3 bandwidth, the
+# denominators when no measured peaks are given
+H100_FP16_DENSE_TFLOPS = 989.0
+H100_HBM_GBPS = 3350.0
 
 
 def load_peaks():
@@ -437,7 +449,7 @@ def run_sharded_predict(args, eng, rank, world, dist):
   if rank == 0:
     per = dev_ms / args.steps
     peaks = load_peaks()
-    tensor_peak = peaks.get("bf16_tflops_sustained") or 1400.0
+    tensor_peak = peaks.get("bf16_tflops_sustained") or H100_FP16_DENSE_TFLOPS
     gemm_ms = stages.get("sc_gemm_nt_planes", 0.0) / args.steps
     # per rank: G/2 of the G^2 block products of the full 2 N^3 flop product (symmetry across ranks)
     flops_rank = 2.0 * n * n * n / (2.0 * world) if world > 1 else 2.0 * n * n * n / 2.0
@@ -461,7 +473,7 @@ def run_sharded_predict(args, eng, rank, world, dist):
         "eigensolve_ms": stages.get("sc_eigh_extremal_sharded", 0.0) / args.steps,
         "stage_ms_rank0": {k: v / args.steps for k, v in sorted(stages.items())},
         "timeline_ms_rank0": refiner_trace,
-        "roofline": {"kernel": "k_gemm_tcgen05 (rank 0's Diffuse block products)", "bound": "tensor",
+        "roofline": {"kernel": "k_gemm_wgmma (rank 0's Diffuse block products)", "bound": "tensor",
                      "achieved": achieved, "peak": tensor_peak, "unit": "TFLOP/s",
                      "frac": (achieved / tensor_peak) if achieved else None, "traffic": None,
                      "note": "achieved = this rank's share of the N^3 triangle-basis flop / CUDA-event "
@@ -573,6 +585,13 @@ def main():
     emb = v[:, :k].contiguous()
     return eng.kmeans(emb, k, 0, clusterer.max_iter)[0]
 
+  def dump_outputs(labels):
+    # the labels predict() returns and the eigenvalues it decided k from (last_details)
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    out = {"labels": labels, "eigenvalues": clusterer.last_details["eigenvalues"]}
+    for name, arr in out.items():
+      np.save(os.path.join(args.dump_outputs, name + ".npy"), np.asarray(arr, dtype=np.float64))
+
   for _ in range(max(1, args.warmup - 2)):     # the e2e loop above already warmed everything
     device_step()
   barrier()
@@ -583,7 +602,7 @@ def main():
   start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
   start.record()
   for _ in range(args.steps):
-    device_step()
+    labels = device_step()
   stop.record()
   barrier()
   dev_ms = start.elapsed_time(stop)
@@ -591,6 +610,8 @@ def main():
   launches = nat.load().sc_launch_count() - launches0
   sampler.stop_flag.set()
   sampler.join(timeout=2)
+  if args.dump_outputs and rank == 0:
+    dump_outputs(labels)
 
   if world > 1:
     tt = torch.tensor([dev_ms, e2e_s], dtype=torch.float64, device=eng.device)
@@ -609,18 +630,12 @@ def main():
     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
   except Exception:
     pass
-  tensor_peak = peaks.get("bf16_tflops_sustained") or 1400.0
+  tensor_peak = peaks.get("bf16_tflops_sustained") or H100_FP16_DENSE_TFLOPS
   peak_note = "measured (MEASURED_PEAKS.json, sustained fp16/bf16 dense)" if peaks else \
-      "fallback (B200_PROFILING.md sustained)"
+      "H100 SXM data sheet, dense fp16 (not a measured rate)"
   diffuse_ms = stages.get("sc_diffuse", 0.0) / args.steps
-  hbm_peak = peaks.get("hbm_gbs") or 6650.0
-  # DRAM traffic of the dominant kernel from the committed `ncu --set full` capture of the same
-  # workload (profiles/traffic.json: {"diffuse_n<N>": bytes per launch}); null when absent.
+  hbm_peak = peaks.get("hbm_gbs") or H100_HBM_GBPS
   traffic = None
-  try:
-    traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get("diffuse_n%d" % n)
-  except Exception:
-    pass
   line = {
       "metric": "embeddings/sec through predict()", "value": value, "unit": "embeddings/s",
       "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_per_step,

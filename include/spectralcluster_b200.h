@@ -1,5 +1,5 @@
 /*
- * spectralcluster_b200 -- C ABI of the B200-native SpectralClusterer.predict() hot path.
+ * spectralcluster_b200 -- C ABI of the H100-native SpectralClusterer.predict() hot path.
  *
  * The reference (wq2012/SpectralCluster v0.2.22) is pure Python and has no FFI:
  * its drop-in boundary is the Python object surface (SURVEY.md 8(b)).  This header
@@ -18,7 +18,7 @@
  *   - `stream` is a cudaStream_t passed as void* (0 = default stream).  Calls are
  *     asynchronous unless stated otherwise.
  *   - "split fp16 planes" (hi, lo): value = hi + lo with hi = fp16(value),
- *     lo = fp16(value - hi): the operand format of the tcgen05 GEMMs (three
+ *     lo = fp16(value - hi): the operand format of the wgmma GEMMs (three
  *     kind::f16 MMAs hi*hi + hi*lo + lo*hi reproduce an fp32-accurate product).
  */
 #ifndef SPECTRALCLUSTER_B200_H_
@@ -40,7 +40,7 @@ enum sc_laplacian_type {                                                        
   SC_LAPLACIAN_RANDOMWALK = 2, SC_LAPLACIAN_GRAPHCUT = 3
 };
 enum sc_gemm_engine {
-  SC_GEMM_TCGEN05 = 0,   /* tcgen05.mma kind::f16 on split planes, TMA-fed (product path) */
+  SC_GEMM_TCGEN05 = 0,   /* tensor cores (wgmma f16) on split planes, TMA-fed (product path) */
   SC_GEMM_SIMT_F64ACC = 1 /* SIMT fp32 operands, fp64 accumulation (validation path, small N) */
 };
 enum sc_gemm_precision {
@@ -145,7 +145,7 @@ int sc_split_planes(sc_context* ctx, const float* a, int64_t n, int64_t lda, voi
                     int64_t ldh, void* stream);
 
 /* Diffuse.refine (refinement.py:232-234): s = y y^T.  rowmax (fp32) / rowsum (fp64), both or
- * neither (tcgen05 engine only), receive max_j s[i,j] and sum_j s[i,j] from the GEMM epilogue: the
+ * neither (tensor-core engine only), receive max_j s[i,j] and sum_j s[i,j] from the GEMM epilogue: the
  * reductions of the following RowWiseNormalize (refinement.py:243) and of the Laplacian degree
  * (laplacian.py:41) without another pass over S.  The fused maximum assumes max_j s[i,j] >= 0,
  * which holds for every y (s[i,i] = |y_i|^2). */
@@ -222,7 +222,7 @@ int sc_scale_shift(sc_context* ctx, const float* x, int64_t ldx, int64_t n, cons
                    const double* col_scale, double alpha, double beta, float* out, int64_t ldo,
                    void* stream);
 /* c[m,n] = a[m,k] b[n,k]^T, fp32 operands, fp64 accumulation (SIMT engine): the products of the
- * propagation (:151-153) for matrices too small for a tcgen05 tile. */
+ * propagation (:151-153) for matrices too small for a tensor-core tile. */
 int sc_gemm_nt_f32(sc_context* ctx, const float* a, int64_t lda, const float* b, int64_t ldb,
                    int64_t m, int64_t n, int64_t k, float* c, int64_t ldc, void* stream);
 

@@ -1,5 +1,5 @@
 """spectralcluster_b200: the SpectralClusterer.predict() hot path of wq2012/SpectralCluster,
-built from scratch for NVIDIA B200 (sm_100a).
+built from scratch for NVIDIA H100 (sm_90a).
 
 The package-level names mirror the reference's import surface for that path
 (/root/reference/spectralcluster/__init__.py:14-43): users switch by changing the import.

@@ -1,6 +1,6 @@
 """ctypes binding of libspectralcluster_b200.so (the C ABI in include/spectralcluster_b200.h).
 
-There is NO CPU fallback: if the library is missing this module raises, and if no B200 is
+There is NO CPU fallback: if the library is missing this module raises, and if no H100 is
 visible `context()` raises.  torch tensors are used only as device buffers (`data_ptr()`).
 """
 

@@ -1,9 +1,9 @@
-"""In-tree build of libspectralcluster_b200.so (sm_100a only).
+"""In-tree build of libspectralcluster_b200.so (sm_90a only).
 
     python -m spectralcluster_b200.build [--force] [--verbose]
 
 nvcc cross-compiles without a GPU.  Objects and the shared library are written to
-spectralcluster_b200/lib/ (git-ignored; the .so travels to the GPU box with the snapshot).
+spectralcluster_b200/lib/ (git-ignored build products).
 """
 
 from __future__ import annotations
@@ -20,7 +20,7 @@ LIBDIR = os.path.join(PKG, "lib")
 LIBNAME = "libspectralcluster_b200.so"
 INCLUDE = os.path.join(os.path.dirname(PKG), "include")
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-O2",
               "--expt-relaxed-constexpr", "-I", INCLUDE]
 

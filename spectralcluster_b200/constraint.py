@@ -6,7 +6,7 @@ ConstraintPropagation's closed form  F = (1-a)^2 (I - a Abar)^-1 Q (I - a Abar)^
 D^-1/2 A D^-1/2) is evaluated on the device without a factorisation: the inverse comes from the
 Newton-Schulz iteration X <- X (2I - M X), M = I - a Abar, which starts at X = I with residual
 a Abar (spectral radius a < 1) and squares it every step -- ceil(log2(ln 1e-9 / ln a)) steps of
-two dense products each, on the same GEMM engines as Diffuse (tcgen05 split-fp16 planes, or the
+two dense products each, on the same GEMM engines as Diffuse (wgmma split-fp16 planes, or the
 SIMT fp64-accumulate engine below 64 rows).  The reference calls np.linalg.inv (:151).
 """
 

@@ -24,12 +24,12 @@ void launched(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int gemm_nt_simt(int epi, const float* A, int64_t lda, const float* B, int64_t ldb, int64_t M,
                  int64_t N, int64_t K, float* C, int64_t ldc, float* rowmax_offdiag,
                  cudaStream_t st);
-// gemm_tcgen05.cu
-int gemm_nt_tcgen05(const sc_context* ctx, int epi, int precision, const __half* a_hi,
-                    const __half* a_lo, int64_t lda, const __half* b_hi, const __half* b_lo,
-                    int64_t ldb, int64_t M, int64_t N, int64_t K, float* C, int64_t ldc,
-                    float* rowmax_offdiag, bool symmetric, int diag_shift, float* stat_rowmax,
-                    double* stat_rowsum, float* mirror, int64_t ldm, cudaStream_t st);
+// gemm_wgmma.cu
+int gemm_nt_wgmma(const sc_context* ctx, int epi, int precision, const __half* a_hi,
+                  const __half* a_lo, int64_t lda, const __half* b_hi, const __half* b_lo,
+                  int64_t ldb, int64_t M, int64_t N, int64_t K, float* C, int64_t ldc,
+                  float* rowmax_offdiag, bool symmetric, int diag_shift, float* stat_rowmax,
+                  double* stat_rowsum, float* mirror, int64_t ldm, cudaStream_t st);
 
 }  // namespace sc
 
@@ -55,8 +55,8 @@ extern "C" int sc_context_create(int device, sc_context** out) {
   SC_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   SC_CUDA(cudaGetDeviceProperties(&prop, device));
-  SC_REQUIRE(prop.major == 10, "sc_context_create: device %d is sm_%d%d; this library is built "
-             "for sm_100a (B200) only", device, prop.major, prop.minor);
+  SC_REQUIRE(prop.major == 9 && prop.minor == 0, "sc_context_create: device %d is sm_%d%d; this "
+             "library is built for sm_90a (H100) only", device, prop.major, prop.minor);
   sc_context* ctx = new sc_context();
   ctx->device = device;
   ctx->sm_count = prop.multiProcessorCount;
@@ -104,8 +104,8 @@ extern "C" int sc_affinity_cosine(sc_context* ctx, int engine, int precision, co
   }
   SC_REQUIRE(engine == SC_GEMM_TCGEN05, "sc_affinity_cosine: unknown engine %d", engine);
   SC_REQUIRE(hi && (lo || precision == SC_GEMM_SINGLE),
-             "sc_affinity_cosine: the tcgen05 engine needs the split fp16 planes");
-  return gemm_nt_tcgen05(ctx, 1, precision, (const __half*)hi, (const __half*)lo, ldh,
+             "sc_affinity_cosine: the tensor-core engine needs the split fp16 planes");
+  return gemm_nt_wgmma(ctx, 1, precision, (const __half*)hi, (const __half*)lo, ldh,
                          (const __half*)hi, (const __half*)lo, ldh, n, n, d, a, lda,
                          rowmax_offdiag, /*symmetric=*/true, /*diag_shift=*/0, nullptr, nullptr,
                          nullptr, 0, as_stream(stream));
@@ -123,12 +123,12 @@ extern "C" int sc_diffuse(sc_context* ctx, int engine, int precision, const floa
   }
   SC_REQUIRE(engine == SC_GEMM_TCGEN05, "sc_diffuse: unknown engine %d", engine);
   SC_REQUIRE(hi && (lo || precision == SC_GEMM_SINGLE),
-             "sc_diffuse: the tcgen05 engine needs the split fp16 planes");
+             "sc_diffuse: the tensor-core engine needs the split fp16 planes");
   if (rowmax) {
     SC_CUDA(cudaMemsetAsync(rowmax, 0, sizeof(float) * n, as_stream(stream)));
     SC_CUDA(cudaMemsetAsync(rowsum, 0, sizeof(double) * n, as_stream(stream)));
   }
-  return gemm_nt_tcgen05(ctx, 0, precision, (const __half*)hi, (const __half*)lo, ldh,
+  return gemm_nt_wgmma(ctx, 0, precision, (const __half*)hi, (const __half*)lo, ldh,
                          (const __half*)hi, (const __half*)lo, ldh, n, n, n, s, lds, nullptr,
                          /*symmetric=*/true, /*diag_shift=*/0, rowmax, rowsum, nullptr, 0,
                          as_stream(stream));
@@ -144,7 +144,7 @@ extern "C" int sc_affinity_cosine_block(sc_context* ctx, int precision, const vo
   SC_REQUIRE(lo || precision == SC_GEMM_SINGLE, "sc_affinity_cosine_block: lo plane missing");
   const __half* h = (const __half*)hi;
   const __half* l = (const __half*)lo;
-  return gemm_nt_tcgen05(ctx, 1, precision, h + row_begin * ldh, l ? l + row_begin * ldh : nullptr,
+  return gemm_nt_wgmma(ctx, 1, precision, h + row_begin * ldh, l ? l + row_begin * ldh : nullptr,
                          ldh, h, l, ldh, row_count, n, d, a_block, lda, rowmax_offdiag_block,
                          /*symmetric=*/false, /*diag_shift=*/(int)row_begin, nullptr, nullptr,
                          nullptr, 0, as_stream(stream));
@@ -158,7 +158,7 @@ extern "C" int sc_gemm_nt_planes(sc_context* ctx, int precision, const void* a_h
   SC_REQUIRE((a_lo && b_lo) || precision == SC_GEMM_SINGLE || (a_lo && precision == SC_GEMM_SPLIT2),
              "sc_gemm_nt_planes: lo planes missing");
   SC_REQUIRE(c_mirror == nullptr || ldm >= m, "sc_gemm_nt_planes: bad mirror leading dimension");
-  return gemm_nt_tcgen05(ctx, 0, precision, (const __half*)a_hi, (const __half*)a_lo, lda,
+  return gemm_nt_wgmma(ctx, 0, precision, (const __half*)a_hi, (const __half*)a_lo, lda,
                          (const __half*)b_hi, (const __half*)b_lo, ldb, m, n, k, c, ldc, nullptr,
                          /*symmetric=*/true, /*diag_shift=*/0, nullptr, nullptr, c_mirror, ldm,
                          as_stream(stream));

@@ -588,7 +588,7 @@ k_blur_band(const BlurArgs g, const BlurWeights bw) {
 
   // tile_is_fast(row0, tx * TTW) for every tile of the band, reduced to four 32-bit compares per
   // tile (the per-tile form -- a dozen 64-bit compares evaluated twice per tile by every thread --
-  // was 17 % of the kernel's instructions, profiles/r02_blur_source_hotspots.txt): the band-level
+  // was a sixth of the kernel's instructions): the band-level
   // conditions once, the first/last tile with a complete halo, and the run of tiles whose halo'd
   // footprint meets the diagonal.
   const bool band_fast = (row0 >= R) && (row0 + TTH + R <= g.n) && (row0 + TTH <= g.row_end) &&
@@ -707,9 +707,9 @@ __device__ __forceinline__ void store_y4(const UpperArgs& g, int64_t i, int64_t 
 }
 
 // (A run-based variant -- one CTA per tile row x 8 tile columns, the next tile's loads prefetched
-// into registers -- measured 5.03 ms against 4.55 ms for this one-tile-per-CTA form on the same box
-// at N = 65,536, profiles/r02_ab_stages_one_box.txt: the extra registers cost more occupancy than
-// the prefetch wins.  The limiter is DRAM page locality of the 128-byte transposed row segments.)
+// into registers -- was slower than this one-tile-per-CTA form: the extra registers cost more
+// occupancy than the prefetch wins.  The limiter is DRAM page locality of the 128-byte transposed
+// row segments.)
 __global__ void __launch_bounds__(256)
 k_thrsym_upper(const UpperArgs g) {
   __shared__ float tile[UT][UT + 1];
@@ -834,9 +834,8 @@ static int launch_blur(const sc_context* ctx, BlurArgs& g, double sigma, cudaStr
       const char* e = getenv("SCB_BLUR_TILES_PER_CTA");
       tpc_env = e ? atoi(e) : 0;
     }
-    // measured (profiles/r02_ab_stages_blur_one_box.txt, N = 65,536): the upper-triangle pass takes
-    // 7.14 / 7.42 / 7.69 / 7.99 ms with runs of 2 / 4 / 8 / 16 tiles (shorter runs balance the ragged
-    // band ends of the triangle); the two-pass kernels keep the 4 of r01_blur_tiles_per_cta_sweep.txt
+    // the upper-triangle pass uses short runs of 2 tiles (they balance the ragged band ends of the
+    // triangle); the two-pass kernels sweep runs of 4
     g.tiles_per_cta = tpc_env > 0 ? tpc_env : (EPI == EPI_UPPER ? 2 : 4);
     if (g.tiles_per_cta > ntiles) g.tiles_per_cta = ntiles;
     const unsigned gy = (unsigned)((ntiles + g.tiles_per_cta - 1) / g.tiles_per_cta);

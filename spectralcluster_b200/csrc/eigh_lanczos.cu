@@ -195,12 +195,11 @@ static int launch_symm(int p, const float* s, int64_t rows, int64_t n, int64_t l
 }
 
 // ---- v2 of the block product: fp64 tensor cores (mma.sync.m8n8k4.f64, SASS DMMA) fed from a
-// cp.async ring (2 stages x 2 CTAs per SM).  Measured on the B200 (profiles/r02_fp64_rate.txt) DMMA and DFMA have the
-// same peak (37 TFLOP/s), but the DFMA form above needs one 64-bit shared load per 4 FMAs of each
-// lane (shared-memory-bound at 1.2x the FP64 pipe) and keeps only 32 KB of loads in flight per SM
-// (ncu: 2.4 TB/s, 14 TFLOP/s).  Here the S tile is staged in shared memory (108 KB in flight per
-// SM), a B fragment (one T value per lane) serves four row groups, and the FP64 pipe is the only
-// busy unit: 16 vectors' worth of DMMA per 4 columns whatever b <= 16 is.
+// cp.async ring (2 stages x 2 CTAs per SM).  The DFMA form above needs one 64-bit shared load per
+// 4 FMAs of each lane (shared-memory-bound) and keeps only 32 KB of loads in flight per SM.  Here
+// the S tile is staged in shared memory (108 KB in flight per SM), a B fragment (one T value per
+// lane) serves four row groups, and the FP64 pipe is the only busy unit: 16 vectors' worth of DMMA
+// per 4 columns whatever b <= 16 is.
 //   CTA = 8 warps x 32 rows (4 row groups of 8) = 256 rows; work item = (row block, column split);
 //   stage = 256 rows x 32 columns of S (fp32, row pitch 36 floats: conflict-free A fragments)
 //         + b vectors x 32 columns of T (fp64, row pitch 36 doubles: conflict-free B fragments).

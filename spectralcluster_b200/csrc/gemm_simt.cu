@@ -1,7 +1,7 @@
 // SIMT validation GEMM: C = A B^T with fp32 operands and fp64 accumulation (every fp32 x fp32
-// product is exact in fp64).  This is NOT the product path for large N -- that is the tcgen05
-// kernel in gemm_tcgen05.cu -- it is the on-device reference the tensor-core kernel is tested
-// against, and the engine used for matrices too small to fill a 128x256 tensor-core tile.
+// product is exact in fp64).  This is NOT the product path for large N -- that is the wgmma
+// kernel in gemm_wgmma.cu -- it is the on-device reference the tensor-core kernel is tested
+// against, and the engine used for matrices too small to fill a 128x128 tensor-core tile.
 //
 //   utils.py:35-39        affinity = (Xn Xn^T + 1) / 2      -> EPI_AFFINITY
 //   refinement.py:232-234 Diffuse: Y Y^T                    -> EPI_PLAIN

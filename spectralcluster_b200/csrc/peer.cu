@@ -2,7 +2,7 @@
 // CUDA IPC handles make a peer rank's Y planes and S row block addressable from this process, so
 //   * the Y row blocks a rank multiplies against are PULLED by the copy engines
 //     (sc_memcpy_async on a side stream: no SM is taken away from the persistent GEMM), and
-//   * the transposed S blocks are PUSHED by the GEMM epilogue itself (k_gemm_tcgen05 `mirror`).
+//   * the transposed S blocks are PUSHED by the GEMM epilogue itself (k_gemm_wgmma `mirror`).
 // The reference has no counterpart (single process, single thread: SURVEY.md section 1).
 #include "common.cuh"
 

@@ -21,13 +21,11 @@ from . import _native as nat
 
 _torch = None
 
-# MMAs per product of the Diffuse GEMM inside predict().  "auto" picks by N from the measured error
-# of each scheme (profiles/r02_diffuse_precision.md): the rounding of the fp16 operand planes is a
-# zero-mean perturbation per product that averages down with sqrt(K) = sqrt(N).  In units of the
-# parity tolerance (|dw| <= 1e-5 |w| + 1e-6 max|w|) the worst eigenvalue error over configs[1],[2]
-# and seeds 0-4 was 0.85 (single) / 0.38 (split2) / 0.014 (split3) at N = 2,400 and 0.33 / 0.15 at
-# N = 16,384 -- labels identical in every run.  So: one MMA from N = 16,384 (<= 1/3 of the
-# tolerance, falling), two from N = 4,096, three below.
+# MMAs per product of the Diffuse GEMM inside predict().  "auto" picks by N from the error of each
+# scheme (tests/diffuse_precision_study.py measures it): the rounding of the fp16 operand planes is
+# a zero-mean perturbation per product that averages down with sqrt(K) = sqrt(N), so the parity
+# tolerance (|dw| <= 1e-5 |w| + 1e-6 max|w|) allows one MMA from N = 16,384, two from N = 4,096 and
+# needs three below (the parity tests pin these sizes).
 DEFAULT_DIFFUSE_PRECISION = "auto"
 AUTO_SINGLE_FROM, AUTO_SPLIT2_FROM = 16384, 4096
 
@@ -53,7 +51,7 @@ class Engine:
 
   _instances: typing.Dict[int, "Engine"] = {}
 
-  # matrices smaller than this use the SIMT fp64-accumulate GEMM (a 128x256 tcgen05 tile would
+  # matrices smaller than this use the SIMT fp64-accumulate GEMM (a 128x128 tensor-core tile would
   # be mostly padding); everything else goes through the tensor-core kernel.
   simt_below = 64
   # force the dense (full-spectrum) eigensolver up to this N even when Lanczos would do (tests)
@@ -63,7 +61,7 @@ class Engine:
     t = torch()
     if not t.cuda.is_available():
       raise RuntimeError(
-          "spectralcluster_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+          "spectralcluster_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     self.device_index = device
     self.device = t.device("cuda", device)
     self.ctx = nat.context(device)
@@ -290,7 +288,7 @@ class Engine:
     return hi, lo
 
   def diffuse(self, n, y=None, hi=None, lo=None, want_stats=False, precision=None):
-    """S = Y Y^T.  With want_stats (tcgen05 engine) also returns (rowmax fp32, rowsum fp64) of S
+    """S = Y Y^T.  With want_stats (tensor-core engine) also returns (rowmax fp32, rowsum fp64) of S
     from the GEMM epilogue; otherwise (None, None).  `precision` defaults to the fp32-accurate
     three-MMA split (the operator-level API); predict() passes `diffuse_precision`."""
     t = torch()

@@ -127,7 +127,7 @@ class Symmetrize(AffinityRefinementOperation):
 
 
 class Diffuse(AffinityRefinementOperation):
-  """A A^T (reference :229-234) on the tcgen05 GEMM."""
+  """A A^T (reference :229-234) on the wgmma GEMM."""
 
   def refine(self, affinity):
     return self._on_device(affinity, lambda eng, a, n: eng.diffuse(n, y=a)[0])

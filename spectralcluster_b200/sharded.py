@@ -298,7 +298,7 @@ class ShardedRefiner:
 
 
 class DeviceBackend:
-  """The CUDA kernels behind the C ABI (tcgen05 GEMMs, fused blur passes)."""
+  """The CUDA kernels behind the C ABI (wgmma GEMMs, fused blur passes)."""
 
   def __init__(self, engine):
     from . import _native as nat

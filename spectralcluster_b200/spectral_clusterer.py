@@ -1,6 +1,6 @@
 """SpectralClusterer -- drop-in mirror of the reference orchestrator
 (/root/reference/spectralcluster/spectral_clusterer.py: __init__ :29-106,
-_compute_eigenvectors_ncluster :108-168, predict :201-314) whose arithmetic runs on a B200.
+_compute_eigenvectors_ncluster :108-168, predict :201-314) whose arithmetic runs on an H100.
 
 predict(): one H2D copy of the [N, d] embeddings, every N x N intermediate stays in HBM
 (affinity GEMM -> fused refinement -> Diffuse GEMM -> row statistics -> symmetric eigensolve ->

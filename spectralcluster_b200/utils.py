@@ -45,7 +45,7 @@ def compute_sorted_eigenvectors(
   scale = np.max(np.abs(m)) if m.size else 0.0
   if m.size and np.max(np.abs(m - m.T)) > 1e-6 * max(scale, 1e-300):
     raise NotImplementedError(
-        "general (non-symmetric) eigendecomposition is outside the B200 hot path "
+        "general (non-symmetric) eigendecomposition is outside the GPU hot path "
         "(SURVEY.md 8(f) rank 1)")
   eng = dev.Engine.get()
   n = m.shape[0]

@@ -16,7 +16,7 @@ _BUILD_ERROR = None
 
 def pytest_configure(config):
   global _BUILD_ERROR
-  config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
+  config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
   # The C-ABI library is a build artefact (git-ignored): make sure it exists and is current
   # before any test imports it (incremental: a no-op when the sources are unchanged).  A box
   # without nvcc can still run the host-logic / oracle tests: the failure is remembered and only
@@ -41,7 +41,7 @@ def _cuda_available():
 def pytest_collection_modifyitems(config, items):
   """`pytest tests` on a machine without CUDA skips the GPU tests instead of failing them."""
   have_gpu = _cuda_available()
-  skip_gpu = pytest.mark.skip(reason="needs a CUDA device (B200); there is no CPU fallback")
+  skip_gpu = pytest.mark.skip(reason="needs a CUDA device (H100); there is no CPU fallback")
   skip_lib = pytest.mark.skip(reason="C-ABI library could not be built: %s" % _BUILD_ERROR)
   for item in items:
     needs_gpu = item.get_closest_marker("gpu") is not None or "engine" in getattr(item, "fixturenames", ())

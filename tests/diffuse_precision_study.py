@@ -6,7 +6,7 @@ For split3 (hi*hi + hi*lo + lo*hi), split2 ((hi+lo)*hi) and single (hi*hi):
     float64 oracle: max relative eigenvalue error over the values the eigengap reads, labels equal?
   * N=16,384, seeds 0-1: element-wise error of 512 sampled rows of S against the float64 product
     (fraction of elements beyond 3e-6, max), eigenvalues against split3, labels against truth.
-Writes a markdown table to stdout (committed as profiles/r02_diffuse_precision.md)."""
+Writes a markdown table to stdout."""
 import os
 import sys
 

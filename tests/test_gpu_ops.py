@@ -127,7 +127,7 @@ def test_diffuse_vs_oracle(n):
   y = rng.random((n, n)).astype(np.float32).astype(np.float64)     # not symmetric on purpose
   want = orc.diffuse(y)
   got = scb.refinement.Diffuse().refine(y)
-  # split-fp16 tcgen05 product: ~2^-22 per term, fp32 accumulation over n terms
+  # split-fp16 tensor-core product: ~2^-22 per term, fp32 accumulation over n terms
   np.testing.assert_allclose(got, want, rtol=3e-6, atol=0)
 
 

@@ -1,4 +1,4 @@
-"""GPU: SpectralClusterer.predict() on the B200 against the golden fixtures produced by the
+"""GPU: SpectralClusterer.predict() on the GPU against the golden fixtures produced by the
 unmodified reference (tests/golden/make_golden.py) and against the oracle run side by side.
 
 Parity bar (BASELINE.json north_star): labels identical after utils.enforce_ordered_labels;

@@ -1,4 +1,4 @@
-"""CPU: host-side logic of the B200 path that needs no GPU -- the symbolic Laplacian terms
+"""CPU: host-side logic of the GPU path that needs no GPU -- the symbolic Laplacian terms
 (SURVEY.md A.2) against the oracle's materialised Laplacians, and the refinement planner's fusion
 decisions against a recording fake engine."""
 

@@ -1,5 +1,6 @@
 """CPU: the oracle reproduces every fixture the unmodified reference produced
-(tests/golden/make_golden.py) -- labels and leading eigenvalues bit for bit."""
+(tests/golden/make_golden.py) -- labels bit for bit, leading eigenvalues to the last few bits
+(LAPACK's rounding depends on the kernels OpenBLAS picks for the host CPU)."""
 
 import numpy as np
 import pytest
@@ -22,4 +23,5 @@ def test_oracle_matches_reference_fixture(name):
   np.testing.assert_array_equal(labels, case["labels"])
   if "eigenvalues_head" in case:
     head = case["eigenvalues_head"]
-    np.testing.assert_array_equal(det["eigenvalues"][:len(head)], head)
+    np.testing.assert_allclose(det["eigenvalues"][:len(head)], head, rtol=1e-11,
+                               atol=1e-12 * np.abs(head).max())

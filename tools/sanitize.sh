@@ -1,5 +1,5 @@
 #!/bin/bash
-# compute-sanitizer racecheck + synccheck on the tcgen05 GEMM (affinity, Diffuse), the cp.async blur
+# compute-sanitizer racecheck + synccheck on the wgmma GEMM (affinity, Diffuse), the cp.async blur
 # pipeline (fused chain), the symmetric blur pair and the block matvec, at small N (VERDICT r01
 # item 9).  Writes gpurun_out/<tag>_sanitizer_{racecheck,synccheck}.txt
 tag=${1:-r02}

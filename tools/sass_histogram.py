@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Opcode histogram of the built library's SASS (cuobjdump -sass), per kernel family: the evidence
-that the hot kernels are Blackwell-native (UTC*MMA = tcgen05.mma, LDTM/STTM = tcgen05.ld/st,
-UTMALDG = TMA loads, LDGSTS = cp.async; no HMMA/HGMMA legacy tensor path).
+that the hot kernels are Hopper-native (HGMMA = wgmma, UTMALDG = TMA loads, SYNCS = mbarrier,
+LDGSTS = cp.async, DMMA = fp64 tensor cores; no HMMA mma.sync fp16 path).
 
-    python tools/sass_histogram.py > profiles/r02_sass_histogram.txt
+    python tools/sass_histogram.py
 """
 import collections
 import os
@@ -13,8 +13,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "spectralcluster_b200", "lib", "libspectralcluster_b200.so")
-INTERESTING = ("UTCHMMA", "UTCQMMA", "UTCBAR", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "LDGSTS",
-               "HMMA", "HGMMA", "DMMA", "DFMA", "FFMA", "FFMA2", "SHFL", "ATOMG", "RED", "SYNCS", "BAR",
+INTERESTING = ("HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UBLKCP", "LDGSTS", "HMMA", "DMMA", "DFMA", "FFMA", "FFMA2", "SHFL", "ATOMG", "RED", "SYNCS", "BAR",
                "LDG", "STG", "LDS", "STS", "MUFU")
 
 out = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
@@ -30,13 +29,12 @@ for line in out.splitlines():
   m = re.match(r"\s+/\*[0-9a-f]{4}\*/\s+(?:@!?U?P\d\s+)?([A-Z0-9_]+)", line)
   if m and name:
     per[name][m.group(1).split(".")[0]] += 1
-print("# SASS opcode histogram of %s (sm_100a), cuobjdump -sass" % os.path.basename(LIB))
+print("# SASS opcode histogram of %s (sm_90a), cuobjdump -sass" % os.path.basename(LIB))
 total = collections.Counter()
 for k, c in per.items():
   total.update(c)
 print("# whole library: " + ", ".join("%s %d" % (op, total[op]) for op in INTERESTING if total[op]))
-print("# legacy tensor path (HMMA/HGMMA/IGMMA/QGMMA): %d instructions" %
-      sum(v for op, v in total.items() if op in ("HMMA", "HGMMA", "IGMMA", "QGMMA")))
+print("# mma.sync fp16 tensor path (HMMA): %d instructions" % total["HMMA"])
 for k, c in per.items():
   n = sum(c.values())
   keys = [op for op in INTERESTING if c[op]]

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Times sc_diffuse (tcgen05 GEMM, Y Y^T) for one N with CUDA events."""
+"""Times sc_diffuse (wgmma GEMM, Y Y^T) for one N with CUDA events."""
 import argparse, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -18,5 +18,5 @@ st.record()
 for _ in range(a.iters): s = eng.diffuse(n, hi=hi, lo=lo, precision=prec)[0]; del s
 en.record(); torch.cuda.synchronize()
 ms = st.elapsed_time(en) / a.iters
-print("N=%d %s 2cta=%s pacing=%s diffuse %.1f ms  %.0f TFLOP/s algorithmic (2N^3)" % (
-    n, a.precision, os.environ.get("SCB_GEMM_2CTA", "1"), "off" if os.environ.get("SCB_NO_GEMM_PACING") else "on", ms, 2.0 * n ** 3 / ms / 1e9))
+print("N=%d %s pacing=%s diffuse %.1f ms  %.0f TFLOP/s algorithmic (2N^3)" % (
+    n, a.precision, "off" if os.environ.get("SCB_NO_GEMM_PACING") else "on", ms, 2.0 * n ** 3 / ms / 1e9))

@@ -2,7 +2,7 @@
 """Per-stage device times (CUDA events around each C-ABI call) of predict() at one N, for A/B runs
 of kernel variants under environment switches on ONE box (box-to-box clocks differ by ~10 %):
 
-    SCB_GEMM_2CTA=0 python tools/time_stages.py --n 65536 --tag 1cta
+    SCB_GEMM_PACE_KB=16 python tools/time_stages.py --n 65536 --tag pace16
 """
 import argparse, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
