@@ -9,16 +9,18 @@
 // 4/3 N^3 tridiagonalisation (>= 47 s of HBM traffic at N = 65,536) is replaced by O(100s) of
 // matrix-vector products, each ONE streaming pass over the fp32 matrix S:
 //
-//   k_symm_f32_f64  Y = S T for a block of b <= 16 vectors: ONE pass over the fp32 matrix per
-//                   block (4 B/element of HBM traffic for b matrix-vector products), fp64 vectors
-//                   staged through shared memory, fp64 accumulation, 4 rows x b vectors of
-//                   register tiling per warp.  A block of b >= (number of wanted pairs) vectors
-//                   also makes the solver find every copy of a repeated eigenvalue (a single
-//                   start vector with full re-orthogonalisation can only ever see one).
-//   k_symv_f32_f64  single-vector variant (kept for b == 1 callers).
-//   k_proj / k_axpy_basis   classical Gram-Schmidt (twice) against the N x m basis
+//   k_symm_dmma + k_symm_reduce   Y = S T for a block of b <= 16 vectors: ONE pass over the fp32
+//                   matrix per block (4 B/element of HBM traffic for b matrix-vector products) on
+//                   the fp64 tensor cores.  A block of b >= (number of wanted pairs) vectors also
+//                   makes the solver find every copy of a repeated eigenvalue (a single start
+//                   vector with full re-orthogonalisation can only ever see one).
+//   k_block_proj / k_block_axpy   block classical Gram-Schmidt (twice) of the b products against
+//                   the N x m basis, then Cholesky-QR (twice) inside the block
+//   k_proj / k_axpy_basis   the same one vector at a time, for a rank-deficient block
 //   k_combine       thick restart V <- V Z
-// The m x m projected problem is solved on the host by cyclic Jacobi (m <= 128).
+// The m x m projected problem (m <= 128) is solved on the host by Householder tridiagonalisation
+// and implicit QL (tred2/tql2).  The sc_krylov_* primitives at the end serve the general
+// (non-symmetric) eigen path of arnoldi.py.
 #include "common.cuh"
 
 #include <algorithm>
@@ -32,6 +34,7 @@ namespace sc {
 constexpr int SYMV_ROWS = 8;       // rows per CTA (one warp each)
 constexpr int SYMV_CHUNK = 2048;   // multiple of 256   // columns of t staged in shared memory per step
 
+// y = S t for one vector: the matrix-vector product of sc_krylov_matvec (general eigen path)
 __global__ void __launch_bounds__(SYMV_ROWS * 32)
 k_symv_f32_f64(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
                const double* __restrict__ t, double* __restrict__ y) {
@@ -66,174 +69,45 @@ k_symv_f32_f64(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds
   if (row < rows && lane == 0) y[row] = acc;
 }
 
-// Y[p][row] = sum_col S[row][col] * T[p][col], p < P: tall-skinny product with the fp32 matrix read
-// once.  CTA = 8 warps x 4 rows.  Software pipeline over chunks of 256 columns: while chunk c is
-// multiplied, the 4 x 8 matrix elements per lane of chunk c+1 are already in flight into a
-// second register set and the T block of chunk c+1 lands in the other shared-memory buffer through
-// cp.async -- one barrier per chunk, no exposed HBM latency (the first version, load-then-use
-// with 1 CTA per SM, ran at 0.9 TB/s).  Lanes walk consecutive columns (coalesced 128 B row
-// segments, conflict-free fp64 shared reads); 4 x P fp64 accumulators per lane, reduced across
-// the warp at the end.
-constexpr int SYMM_ROWS_PER_WARP = 4;
-constexpr int SYMM_WARPS = 8;
-constexpr int SYMM_CHUNK = 256;    // columns per pipeline step: 2 buffers x P x 256 x 8 B <= 64 KB
-constexpr int SYMM_ITERS = SYMM_CHUNK / 32;
-
-template <int P>
-__global__ void __launch_bounds__(SYMM_WARPS * 32, 1)
-k_symm_f32_f64(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
-               const double* __restrict__ t /*[P][ldt]*/, int64_t ldt,
-               double* __restrict__ y /*[P][ldy]*/, int64_t ldy) {
-  extern __shared__ double ts_raw[];                 // [2][P][SYMM_CHUNK]
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t row0 = ((int64_t)blockIdx.x * SYMM_WARPS + warp) * SYMM_ROWS_PER_WARP;
-  const float* r[SYMM_ROWS_PER_WARP];
-#pragma unroll
-  for (int q = 0; q < SYMM_ROWS_PER_WARP; ++q) r[q] = s + (row0 + q < rows ? row0 + q : 0) * lds;
-  double acc[SYMM_ROWS_PER_WARP][P];
-#pragma unroll
-  for (int q = 0; q < SYMM_ROWS_PER_WARP; ++q)
-#pragma unroll
-    for (int p = 0; p < P; ++p) acc[q][p] = 0.0;
-  const int64_t chunks = (n + SYMM_CHUNK - 1) / SYMM_CHUNK;
-  // the T block is copied 16 bytes (2 doubles) at a time: ldt is even and t 16-byte aligned (the
-  // host pads); a last odd column goes through the scalar branch, columns past n read as zero
-  auto stage_t = [&](int64_t c, int buf) {
-    double* dst = ts_raw + (size_t)buf * P * SYMM_CHUNK;
-    const int64_t c0 = c * SYMM_CHUNK;
-    for (int idx = threadIdx.x; idx < P * (SYMM_CHUNK / 2); idx += SYMM_WARPS * 32) {
-      const int p = idx / (SYMM_CHUNK / 2), j2 = (idx - p * (SYMM_CHUNK / 2)) * 2;
-      double* d2 = dst + p * SYMM_CHUNK + j2;
-      if (c0 + j2 + 1 < n) {
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;"
-                     ::"r"((uint32_t)__cvta_generic_to_shared(d2)), "l"(t + (int64_t)p * ldt + c0 + j2)
-                     : "memory");
-      } else {
-        d2[0] = (c0 + j2 < n) ? t[(int64_t)p * ldt + c0 + j2] : 0.0;
-        d2[1] = 0.0;
-      }
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  };
-  auto load_s = [&](int64_t c, float (&q4)[SYMM_ITERS][SYMM_ROWS_PER_WARP]) {
-    const int64_t c0 = c * SYMM_CHUNK;
-#pragma unroll
-    for (int it = 0; it < SYMM_ITERS; ++it) {
-      const int64_t j = c0 + it * 32 + lane;
-#pragma unroll
-      for (int q = 0; q < SYMM_ROWS_PER_WARP; ++q)
-        q4[it][q] = (j < n) ? ld_stream1(r[q] + j) : 0.0f;
-    }
-  };
-  auto multiply = [&](const float (&q4)[SYMM_ITERS][SYMM_ROWS_PER_WARP], int buf) {
-    const double* ts = ts_raw + (size_t)buf * P * SYMM_CHUNK;
-#pragma unroll
-    for (int it = 0; it < SYMM_ITERS; ++it) {
-#pragma unroll
-      for (int p = 0; p < P; ++p) {
-        const double tv = ts[p * SYMM_CHUNK + it * 32 + lane];
-#pragma unroll
-        for (int q = 0; q < SYMM_ROWS_PER_WARP; ++q) acc[q][p] = fma((double)q4[it][q], tv, acc[q][p]);
-      }
-    }
-  };
-  float sa[SYMM_ITERS][SYMM_ROWS_PER_WARP], sb[SYMM_ITERS][SYMM_ROWS_PER_WARP];
-  stage_t(0, 0);
-  load_s(0, sa);
-  for (int64_t c = 0; c < chunks; c += 2) {
-    // ---- even chunk: registers `sa`, buffer 0; prefetch chunk c+1 into `sb`, buffer 1
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncthreads();                       // buffer 0 landed; everybody has left buffer 1
-    if (c + 1 < chunks) {
-      stage_t(c + 1, 1);
-      load_s(c + 1, sb);
-    }
-    multiply(sa, 0);
-    if (c + 1 >= chunks) break;
-    // ---- odd chunk: registers `sb`, buffer 1; prefetch chunk c+2 into `sa`, buffer 0
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncthreads();
-    if (c + 2 < chunks) {
-      stage_t(c + 2, 0);
-      load_s(c + 2, sa);
-    }
-    multiply(sb, 1);
-  }
-#pragma unroll
-  for (int q = 0; q < SYMM_ROWS_PER_WARP; ++q)
-#pragma unroll
-    for (int p = 0; p < P; ++p) {
-      const double v = warp_sum(acc[q][p]);
-      if (lane == 0 && row0 + q < rows) y[(int64_t)p * ldy + row0 + q] = v;
-    }
-}
-
-template <int P>
-static int launch_symm_p(const float* s, int64_t rows, int64_t n, int64_t lds, const double* t,
-                         int64_t ldt, double* y, int64_t ldy, cudaStream_t st) {
-  const unsigned grid = (unsigned)((rows + SYMM_WARPS * SYMM_ROWS_PER_WARP - 1) /
-                                   (SYMM_WARPS * SYMM_ROWS_PER_WARP));
-  const size_t smem = sizeof(double) * 2 * P * SYMM_CHUNK;
-  auto kern = k_symm_f32_f64<P>;
-  SC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<grid, SYMM_WARPS * 32, smem, st>>>(s, rows, n, lds, t, ldt, y, ldy);
-  sc::launched();
-  return 0;
-}
-
-static int launch_symm(int p, const float* s, int64_t rows, int64_t n, int64_t lds, const double* t,
-                       int64_t ldt, double* y, int64_t ldy, cudaStream_t st) {
-  SC_REQUIRE((reinterpret_cast<uintptr_t>(t) & 15) == 0 && ldt % 2 == 0 && ldt >= n,
-             "sc_eigh_extremal: internal (the block product wants an even ldt and an aligned T)");
-  switch (p) {
-    case 4: return launch_symm_p<4>(s, rows, n, lds, t, ldt, y, ldy, st);
-    case 8: return launch_symm_p<8>(s, rows, n, lds, t, ldt, y, ldy, st);
-    case 12: return launch_symm_p<12>(s, rows, n, lds, t, ldt, y, ldy, st);
-    case 16: return launch_symm_p<16>(s, rows, n, lds, t, ldt, y, ldy, st);
-    default: set_error("sc_eigh_extremal: unsupported block size %d", p); return 2;
-  }
-}
-
-// ---- v2 of the block product: fp64 tensor cores (mma.sync.m8n8k4.f64, SASS DMMA) fed from a
-// cp.async ring (2 stages x 2 CTAs per SM).  The DFMA form above needs one 64-bit shared load per
-// 4 FMAs of each lane (shared-memory-bound) and keeps only 32 KB of loads in flight per SM.  Here
-// the S tile is staged in shared memory (108 KB in flight per SM), a B fragment (one T value per
-// lane) serves four row groups, and the FP64 pipe is the only busy unit: 16 vectors' worth of DMMA
-// per 4 columns whatever b <= 16 is.
+// ---- block product: fp64 tensor cores (mma.sync.m8n8k4.f64, SASS DMMA) fed from a cp.async ring
+// (2 stages x 2 CTAs per SM).  A DFMA form needs one 64-bit shared load per 4 FMAs of each lane
+// (shared-memory-bound); here the S tile is staged in shared memory (108 KB in flight per SM), a B
+// fragment (one T value per lane) serves four row groups, and the FP64 pipe is the only busy unit:
+// 16 vectors' worth of DMMA per 4 columns whatever b <= 16 is.
 //   CTA = 8 warps x 32 rows (4 row groups of 8) = 256 rows; work item = (row block, column split);
 //   stage = 256 rows x 32 columns of S (fp32, row pitch 36 floats: conflict-free A fragments)
 //         + b vectors x 32 columns of T (fp64, row pitch 36 doubles: conflict-free B fragments).
 //   Column splits keep >= ~6 work items per SM; their partial products are summed in a fixed order
 //   by k_symm_reduce (every rank of a sharded run must get bit-identical vectors).
-constexpr int S2_ROWS = 256, S2_COLS = 32, S2_SP = 36, S2_TP = 36, S2_MAXB = 16;
-constexpr int S2_S_FLOATS = S2_ROWS * S2_SP;                       // 9,216 floats = 36,864 B
-constexpr int S2_STAGE_BYTES = S2_S_FLOATS * 4 + S2_MAXB * S2_TP * 8;   // + 4,608 B
+constexpr int SYMM_ROWS = 256, SYMM_COLS = 32, SYMM_SP = 36, SYMM_TP = 36, SYMM_MAXB = 16;
+constexpr int SYMM_S_FLOATS = SYMM_ROWS * SYMM_SP;                       // 9,216 floats = 36,864 B
+constexpr int SYMM_STAGE_BYTES = SYMM_S_FLOATS * 4 + SYMM_MAXB * SYMM_TP * 8;   // + 4,608 B
+constexpr int SYMM_STAGES = 2;     // x 41,472 B: two CTAs (16 warps) per SM
 
 __device__ __forceinline__ void cp_async16_zfill(void* dst, const void* src, int src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;"
                ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src), "r"(src_bytes) : "memory");
 }
 
-template <int S2_STAGES>       // 2 stages: two CTAs per SM (16 warps, the default); 4: one CTA per SM
-__global__ void __launch_bounds__(256, S2_STAGES <= 2 ? 2 : 1)
+__global__ void __launch_bounds__(256, 2)
 k_symm_dmma(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
             const double* __restrict__ t /*[b][ldt]*/, int64_t ldt, int b, int row_blocks,
             int64_t cols_per_split, double* __restrict__ partial /*[split][b][rows_pad]*/,
             int64_t rows_pad) {
-  extern __shared__ __align__(16) unsigned char s2_smem[];
+  extern __shared__ __align__(16) unsigned char symm_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rb = blockIdx.x % row_blocks, split = blockIdx.x / row_blocks;
-  const int64_t row0 = (int64_t)rb * S2_ROWS;
+  const int64_t row0 = (int64_t)rb * SYMM_ROWS;
   const int64_t c_begin = (int64_t)split * cols_per_split;
   const int64_t c_end = min(n, c_begin + cols_per_split);
-  const int chunks = (int)((c_end - c_begin + S2_COLS - 1) / S2_COLS);
-  auto stage_s = [&](int st) { return reinterpret_cast<float*>(s2_smem + (size_t)st * S2_STAGE_BYTES); };
+  const int chunks = (int)((c_end - c_begin + SYMM_COLS - 1) / SYMM_COLS);
+  auto stage_s = [&](int st) { return reinterpret_cast<float*>(symm_smem + (size_t)st * SYMM_STAGE_BYTES); };
   auto stage_t = [&](int st) {
-    return reinterpret_cast<double*>(s2_smem + (size_t)st * S2_STAGE_BYTES + S2_S_FLOATS * 4);
+    return reinterpret_cast<double*>(symm_smem + (size_t)st * SYMM_STAGE_BYTES + SYMM_S_FLOATS * 4);
   };
   // fill: 256 rows x 8 16-byte granules of S (8 per thread), b rows x 16 granules of T
   auto fill = [&](int ch, int st) {
-    const int64_t c0 = c_begin + (int64_t)ch * S2_COLS;
+    const int64_t c0 = c_begin + (int64_t)ch * SYMM_COLS;
     float* ss = stage_s(st);
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
@@ -243,7 +117,7 @@ k_symm_dmma(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
       const int64_t gc = c0 + 4 * q;
       int64_t valid = c_end - gc;
       valid = valid < 0 ? 0 : (valid > 4 ? 4 : valid);
-      cp_async16_zfill(ss + r * S2_SP + 4 * q, s + gr * lds + (valid > 0 ? gc : 0), (int)valid * 4);
+      cp_async16_zfill(ss + r * SYMM_SP + 4 * q, s + gr * lds + (valid > 0 ? gc : 0), (int)valid * 4);
     }
     double* ts = stage_t(st);
     for (int idx = threadIdx.x; idx < b * 16; idx += 256) {
@@ -251,7 +125,7 @@ k_symm_dmma(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
       const int64_t gc = c0 + 2 * q;
       int64_t valid = c_end - gc;
       valid = valid < 0 ? 0 : (valid > 2 ? 2 : valid);
-      cp_async16_zfill(ts + p * S2_TP + 2 * q, t + (int64_t)p * ldt + (valid > 0 ? gc : 0), (int)valid * 8);
+      cp_async16_zfill(ts + p * SYMM_TP + 2 * q, t + (int64_t)p * ldt + (valid > 0 ? gc : 0), (int)valid * 8);
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   };
@@ -265,24 +139,24 @@ k_symm_dmma(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
   const bool n0_live = fr < b;
   const bool two_tiles = b > 8;                         // block-uniform
 #pragma unroll
-  for (int st = 0; st < S2_STAGES - 1; ++st) {
+  for (int st = 0; st < SYMM_STAGES - 1; ++st) {
     if (st < chunks) fill(st, st);
     else asm volatile("cp.async.commit_group;" ::: "memory");
   }
   for (int ch = 0; ch < chunks; ++ch) {
-    asm volatile("cp.async.wait_group %0;" ::"n"(S2_STAGES - 2) : "memory");
+    asm volatile("cp.async.wait_group %0;" ::"n"(SYMM_STAGES - 2) : "memory");
     __syncthreads();                                    // chunk ch landed; stage (ch-1)%S is free
-    if (ch + S2_STAGES - 1 < chunks) fill(ch + S2_STAGES - 1, (ch + S2_STAGES - 1) % S2_STAGES);
+    if (ch + SYMM_STAGES - 1 < chunks) fill(ch + SYMM_STAGES - 1, (ch + SYMM_STAGES - 1) % SYMM_STAGES);
     else asm volatile("cp.async.commit_group;" ::: "memory");
-    const float* ss = stage_s(ch % S2_STAGES) + (warp * 32 + fr) * S2_SP + fk;
-    const double* ts = stage_t(ch % S2_STAGES) + fk;
+    const float* ss = stage_s(ch % SYMM_STAGES) + (warp * 32 + fr) * SYMM_SP + fk;
+    const double* ts = stage_t(ch % SYMM_STAGES) + fk;
 #pragma unroll
-    for (int ks = 0; ks < S2_COLS / 4; ++ks) {
-      const double b0 = n0_live ? ts[fr * S2_TP + 4 * ks] : 0.0;
-      const double b1 = n1_live ? ts[(8 + fr) * S2_TP + 4 * ks] : 0.0;
+    for (int ks = 0; ks < SYMM_COLS / 4; ++ks) {
+      const double b0 = n0_live ? ts[fr * SYMM_TP + 4 * ks] : 0.0;
+      const double b1 = n1_live ? ts[(8 + fr) * SYMM_TP + 4 * ks] : 0.0;
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
-        const double a = (double)ss[g * 8 * S2_SP + 4 * ks];
+        const double a = (double)ss[g * 8 * SYMM_SP + 4 * ks];
         asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
                      : "+d"(acc[g][0][0]), "+d"(acc[g][0][1]) : "d"(a), "d"(b0));
         if (two_tiles)                                  // b <= 8: the second n-tile would be all zeros
@@ -318,16 +192,16 @@ __global__ void k_symm_reduce(const double* __restrict__ partial, int splits, in
   y[(int64_t)p * ldy + row] = acc;
 }
 
-// scratch the caller provides for the v2 product: doubles
-static size_t symm_v2_scratch_doubles(int64_t rows, int64_t n, int b, int sm_count, int* splits_out,
-                                      int64_t* cols_per_split_out) {
-  const int64_t row_blocks = (rows + S2_ROWS - 1) / S2_ROWS;
+// scratch the caller provides for the block product: doubles
+static size_t block_product_scratch_doubles(int64_t rows, int64_t n, int b, int sm_count,
+                                            int* splits_out, int64_t* cols_per_split_out) {
+  const int64_t row_blocks = (rows + SYMM_ROWS - 1) / SYMM_ROWS;
   int64_t splits = (6LL * sm_count + row_blocks - 1) / row_blocks;
   const int64_t max_splits = (n + 2047) / 2048;           // at least 2,048 columns per work item
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;
   int64_t cps = (n + splits - 1) / splits;
-  cps = (cps + S2_COLS - 1) / S2_COLS * S2_COLS;
+  cps = (cps + SYMM_COLS - 1) / SYMM_COLS * SYMM_COLS;
   splits = (n + cps - 1) / cps;
   *splits_out = (int)splits;
   *cols_per_split_out = cps;
@@ -335,24 +209,20 @@ static size_t symm_v2_scratch_doubles(int64_t rows, int64_t n, int b, int sm_cou
   return (size_t)splits * b * rows_pad;
 }
 
-static int launch_symm_v2(int b, const float* s, int64_t rows, int64_t n, int64_t lds, const double* t,
-                          int64_t ldt, double* y, int64_t ldy, double* scratch, int splits,
-                          int64_t cols_per_split, cudaStream_t st) {
-  SC_REQUIRE(b >= 1 && b <= S2_MAXB && ldt % 2 == 0 && (reinterpret_cast<uintptr_t>(t) & 15) == 0 &&
+// Y = S T (k_symm_dmma, then k_symm_reduce); `scratch`, `splits` and `cols_per_split` come from
+// block_product_scratch_doubles
+static int launch_block_product(int b, const float* s, int64_t rows, int64_t n, int64_t lds,
+                                const double* t, int64_t ldt, double* y, int64_t ldy, double* scratch,
+                                int splits, int64_t cols_per_split, cudaStream_t st) {
+  SC_REQUIRE(b >= 1 && b <= SYMM_MAXB && ldt % 2 == 0 && (reinterpret_cast<uintptr_t>(t) & 15) == 0 &&
              lds % 4 == 0 && (reinterpret_cast<uintptr_t>(s) & 15) == 0,
              "sc_eigh_extremal: internal (block product alignment)");
-  const int row_blocks = (int)((rows + S2_ROWS - 1) / S2_ROWS);
+  const int row_blocks = (int)((rows + SYMM_ROWS - 1) / SYMM_ROWS);
   const int64_t rows_pad = (rows + 1) & ~(int64_t)1;
-  static int stages = 0;
-  if (stages == 0) {
-    const char* e = getenv("SCB_SYMM_STAGES");
-    stages = (e && atoi(e) == 4) ? 4 : 2;    // measured: 18.4 vs 21.3 ms per solve at N = 65,536
-  }
-  const size_t smem = (size_t)stages * S2_STAGE_BYTES;
-  auto kern = stages == 2 ? k_symm_dmma<2> : k_symm_dmma<4>;
-  SC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<(unsigned)(row_blocks * splits), 256, smem, st>>>(s, rows, n, lds, t, ldt, b, row_blocks,
-                                                         cols_per_split, scratch, rows_pad);
+  const size_t smem = (size_t)SYMM_STAGES * SYMM_STAGE_BYTES;
+  SC_CUDA(cudaFuncSetAttribute(k_symm_dmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_symm_dmma<<<(unsigned)(row_blocks * splits), 256, smem, st>>>(s, rows, n, lds, t, ldt, b, row_blocks,
+                                                                cols_per_split, scratch, rows_pad);
   sc::launched();
   k_symm_reduce<<<dim3((unsigned)((rows + 255) / 256), (unsigned)b), 256, 0, st>>>(scratch, splits, b, rows,
                                                                                  rows_pad, y, ldy);
@@ -414,6 +284,31 @@ __global__ void k_norm2(const double* __restrict__ w, int64_t n, double* __restr
   for (int64_t i = threadIdx.x; i < n; i += blockDim.x) s = fma(w[i], w[i], s);
   s = block_sum(s, red);
   if (threadIdx.x == 0) out[0] = s;
+}
+
+// w (device, length n) <- w orthogonalised against the cnt basis vectors v[0..cnt) by classical
+// Gram-Schmidt applied twice; h1 / h2 (device, cnt each) take the coefficients of the two sweeps and
+// nrm (device) the squared norm of what is left.  Copies h1, h2 to h1_host, h2_host when those are
+// given and the norm to *nrm2_host.  One stream synchronisation.
+static int gram_schmidt2(const double* v, int64_t n, int cnt, double* w, double* h1, double* h2,
+                         double* nrm, double* h1_host, double* h2_host, double* nrm2_host,
+                         cudaStream_t st) {
+  const unsigned gn = (unsigned)((n + 255) / 256);
+  if (cnt > 0) {
+    k_proj<<<(unsigned)cnt, 256, 0, st>>>(v, n, w, h1); sc::launched();
+    k_axpy_basis<<<gn, 256, 0, st>>>(v, n, cnt, h1, w); sc::launched();
+    k_proj<<<(unsigned)cnt, 256, 0, st>>>(v, n, w, h2); sc::launched();
+    k_axpy_basis<<<gn, 256, 0, st>>>(v, n, cnt, h2, w); sc::launched();
+  }
+  k_norm2<<<1, 1024, 0, st>>>(w, n, nrm); sc::launched();
+  SC_LAUNCH_CHECK();
+  if (h1_host && cnt > 0) {
+    SC_CUDA(cudaMemcpyAsync(h1_host, h1, sizeof(double) * cnt, cudaMemcpyDeviceToHost, st));
+    SC_CUDA(cudaMemcpyAsync(h2_host, h2, sizeof(double) * cnt, cudaMemcpyDeviceToHost, st));
+  }
+  SC_CUDA(cudaMemcpyAsync(nrm2_host, nrm, sizeof(double), cudaMemcpyDeviceToHost, st));
+  SC_CUDA(cudaStreamSynchronize(st));
+  return 0;
 }
 
 __global__ void k_scale_into(const double* __restrict__ w, int64_t n, double alpha,
@@ -752,8 +647,9 @@ typedef int (*sc_gather_fn)(void* user, int count);
 //
 // Band (block) Lanczos with full re-orthogonalisation.  Basis v_0..v_{J-1}; the operator has been
 // applied to the first P of them ("processed"), J = P + b.  One step multiplies the block
-// v_P..v_{P+b-1} (ONE pass over S), then orthogonalises the b products one at a time against the
-// whole basis (classical Gram-Schmidt, twice), each giving one new basis vector.  T = V^T Op V is
+// v_P..v_{P+b-1} (ONE pass over S), then orthogonalises the b products against the whole basis
+// (block classical Gram-Schmidt, twice) and among themselves (Cholesky-QR, twice), giving b new
+// basis vectors; a rank-deficient block goes one vector at a time instead.  T = V^T Op V is
 // banded (plus the arrow left by a thick restart); Ritz pairs come from T[0:P,0:P], their
 // residuals from the coupling rows T[P:P+b, 0:P].
 static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t row_begin,
@@ -814,30 +710,12 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   double nrm2 = 0.0;
   uint64_t reseed = 1;
 
-  // w (device, length n) <- w orthogonalised twice against V[0..cnt); hh += coefficients; returns
-  // its squared norm in nrm2 (host).  One stream synchronisation.
-  auto orthogonalise = [&](double* w, int cnt, bool want_h) -> int {
-    if (cnt > 0) {
-      k_proj<<<cnt, 256, 0, st>>>(V, n, w, h_dev); sc::launched();
-      k_axpy_basis<<<gn, 256, 0, st>>>(V, n, cnt, h_dev, w); sc::launched();
-      k_proj<<<cnt, 256, 0, st>>>(V, n, w, h2_dev); sc::launched();
-      k_axpy_basis<<<gn, 256, 0, st>>>(V, n, cnt, h2_dev, w); sc::launched();
-    }
-    k_norm2<<<1, 1024, 0, st>>>(w, n, nrm_dev); sc::launched();
-    SC_LAUNCH_CHECK();
-    if (want_h && cnt > 0) {
-      SC_CUDA(cudaMemcpyAsync(hh.data(), h_dev, sizeof(double) * cnt, cudaMemcpyDeviceToHost, st));
-      SC_CUDA(cudaMemcpyAsync(hh2.data(), h2_dev, sizeof(double) * cnt, cudaMemcpyDeviceToHost, st));
-    }
-    SC_CUDA(cudaMemcpyAsync(&nrm2, nrm_dev, sizeof(double), cudaMemcpyDeviceToHost, st));
-    SC_CUDA(cudaStreamSynchronize(st));
-    return 0;
-  };
   // V[at] <- a fresh random direction orthogonal to V[0..at)
   auto random_direction = [&](int at) -> int {
     double* w = wb;                                  // scratch: callers are done with wb[0]
     k_random_vec<<<gn, 256, 0, st>>>(w, n, 0x5CB200ull + 7919ull * reseed++); sc::launched();
-    if (int rc = orthogonalise(w, at, false)) return rc;
+    if (int rc = gram_schmidt2(V, n, at, w, h_dev, h2_dev, nrm_dev, nullptr, nullptr, &nrm2, st))
+      return rc;
     k_scale_into<<<gn, 256, 0, st>>>(w, n, 1.0 / std::sqrt(nrm2), V + (size_t)at * n); sc::launched();
     return 0;
   };
@@ -890,20 +768,11 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   }
 
   const bool trace = std::getenv("SCB_LANCZOS_TRACE") != nullptr;
-  // block product: DMMA kernel (v2) unless SCB_SYMM_V2=0
-  static int symm_v2_mode = -1;
-  if (symm_v2_mode < 0) {
-    const char* e = std::getenv("SCB_SYMM_V2");
-    symm_v2_mode = (e && std::atoi(e) == 0) ? 0 : 1;
-  }
-  const bool symm_v2 = symm_v2_mode == 1;
-  int v2_splits = 1;
-  int64_t v2_cols = n;
-  Scratch v2buf;
-  if (symm_v2) {
-    const size_t need = symm_v2_scratch_doubles(rows, n, b, ctx->sm_count, &v2_splits, &v2_cols);
-    SC_CUDA(v2buf.alloc(sizeof(double) * need, st));
-  }
+  int prod_splits = 1;
+  int64_t prod_cols = n;
+  Scratch prod_buf;
+  SC_CUDA(prod_buf.alloc(sizeof(double) * block_product_scratch_doubles(rows, n, b, ctx->sm_count,
+                                                                        &prod_splits, &prod_cols), st));
   int P = 0, J = b;
   int64_t matvecs = 0, restarts = 0, passes = 0;
   int converged = 0, mm = 0;
@@ -951,12 +820,8 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   for (;;) {
     // ---- one pass over S: W = flip * Op V[P..P+b)
     k_prescale<<<dim3(gn, b), 256, 0, st>>>(V + (size_t)P * n, left, right, n, tb, ldtb); sc::launched();
-    if (symm_v2) {
-      if (int rc = launch_symm_v2(b, s, rows, n, lds, tb, ldtb, y_mine, y_slab_len, v2buf.as<double>(),
-                                  v2_splits, v2_cols, st)) return rc;
-    } else {
-      if (int rc = launch_symm(b, s, rows, n, lds, tb, ldtb, y_mine, y_slab_len, st)) return rc;
-    }
+    if (int rc = launch_block_product(b, s, rows, n, lds, tb, ldtb, y_mine, y_slab_len,
+                                      prod_buf.as<double>(), prod_splits, prod_cols, st)) return rc;
     SC_LAUNCH_CHECK();
     if (gather) SC_REQUIRE(gather(user, b) == 0, "sc_eigh_extremal_sharded: the gather callback failed");
     k_postscale<<<dim3(gn, b), 256, 0, st>>>(V + (size_t)P * n, y_base, y_slab_len, b, delta, left,
@@ -995,7 +860,8 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
     for (int p = 0; p < b && qr_status != 0; ++p) {
       double* w = wb + (size_t)p * n;
       const int col = P + p;
-      if (int rc = orthogonalise(w, J, true)) return rc;
+      if (int rc = gram_schmidt2(V, n, J, w, h_dev, h2_dev, nrm_dev, hh.data(), hh2.data(), &nrm2, st))
+        return rc;
       for (int q = 0; q < J; ++q) {
         const double v = hh[q] + hh2[q];
         Tat(q, col) += v;
@@ -1082,14 +948,14 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
 extern "C" int sc_block_product(sc_context* ctx, const float* s, int64_t rows, int64_t n, int64_t lds,
                                 const double* t, int64_t ldt, int b, double* y, int64_t ldy,
                                 void* stream) {
-  SC_REQUIRE(ctx && s && t && y && rows > 0 && n > 0 && b >= 1 && b <= S2_MAXB && ldt >= n && ldy >= rows,
+  SC_REQUIRE(ctx && s && t && y && rows > 0 && n > 0 && b >= 1 && b <= SYMM_MAXB && ldt >= n && ldy >= rows,
              "sc_block_product: bad arguments");
   cudaStream_t st = as_stream(stream);
   int splits = 1;
   int64_t cols = n;
   Scratch buf;
-  SC_CUDA(buf.alloc(sizeof(double) * symm_v2_scratch_doubles(rows, n, b, ctx->sm_count, &splits, &cols), st));
-  if (int rc = launch_symm_v2(b, s, rows, n, lds, t, ldt, y, ldy, buf.as<double>(), splits, cols, st)) return rc;
+  SC_CUDA(buf.alloc(sizeof(double) * block_product_scratch_doubles(rows, n, b, ctx->sm_count, &splits, &cols), st));
+  if (int rc = launch_block_product(b, s, rows, n, lds, t, ldt, y, ldy, buf.as<double>(), splits, cols, st)) return rc;
   SC_LAUNCH_CHECK();
   return 0;
 }
@@ -1154,22 +1020,9 @@ extern "C" int sc_krylov_orthogonalize(sc_context* ctx, const double* v, int64_t
   double* h1 = small.as<double>();
   double* h2 = h1 + count;
   double* nrm = h2 + count;
-  const unsigned gn = (unsigned)((n + 255) / 256);
   std::vector<double> a((size_t)count), b((size_t)count);
-  if (count > 0) {
-    k_proj<<<(unsigned)count, 256, 0, st>>>(v, n, w, h1); sc::launched();
-    k_axpy_basis<<<gn, 256, 0, st>>>(v, n, (int)count, h1, w); sc::launched();
-    k_proj<<<(unsigned)count, 256, 0, st>>>(v, n, w, h2); sc::launched();
-    k_axpy_basis<<<gn, 256, 0, st>>>(v, n, (int)count, h2, w); sc::launched();
-  }
-  k_norm2<<<1, 1024, 0, st>>>(w, n, nrm); sc::launched();
-  SC_LAUNCH_CHECK();
-  if (count > 0) {
-    SC_CUDA(cudaMemcpyAsync(a.data(), h1, sizeof(double) * count, cudaMemcpyDeviceToHost, st));
-    SC_CUDA(cudaMemcpyAsync(b.data(), h2, sizeof(double) * count, cudaMemcpyDeviceToHost, st));
-  }
-  SC_CUDA(cudaMemcpyAsync(nrm2_host, nrm, sizeof(double), cudaMemcpyDeviceToHost, st));
-  SC_CUDA(cudaStreamSynchronize(st));
+  if (int rc = gram_schmidt2(v, n, (int)count, w, h1, h2, nrm, a.data(), b.data(), nrm2_host, st))
+    return rc;
   for (int64_t q = 0; q < count; ++q) h_host[q] = a[q] + b[q];
   return 0;
 }

@@ -21,12 +21,11 @@ from . import _native as nat
 
 _torch = None
 
-# MMAs per product of the Diffuse GEMM inside predict().  "auto" picks by N from the error of each
-# scheme (tests/diffuse_precision_study.py measures it): the rounding of the fp16 operand planes is
-# a zero-mean perturbation per product that averages down with sqrt(K) = sqrt(N), so the parity
+# MMAs per product of the Diffuse GEMM inside predict(), picked by N from the error of each scheme
+# (tests/diffuse_precision_study.py measures it): the rounding of the fp16 operand planes is a
+# zero-mean perturbation per product that averages down with sqrt(K) = sqrt(N), so the parity
 # tolerance (|dw| <= 1e-5 |w| + 1e-6 max|w|) allows one MMA from N = 16,384, two from N = 4,096 and
 # needs three below (the parity tests pin these sizes).
-DEFAULT_DIFFUSE_PRECISION = "auto"
 AUTO_SINGLE_FROM, AUTO_SPLIT2_FROM = 16384, 4096
 
 
@@ -66,11 +65,9 @@ class Engine:
     self.device = t.device("cuda", device)
     self.ctx = nat.context(device)
     self.gemm_precision = nat.GEMM_SPLIT3       # affinity: its entries feed a threshold
-    # Diffuse inside predict() (K = N): MMAs per product, SCB_DIFFUSE_PRECISION = split3 | split2
-    # | single.  The operator-level API (refinement.Diffuse) always uses split3.
-    self.diffuse_precision = {"auto": None, "split3": nat.GEMM_SPLIT3, "split2": nat.GEMM_SPLIT2,
-                              "single": nat.GEMM_SINGLE}[
-                                  os.environ.get("SCB_DIFFUSE_PRECISION", DEFAULT_DIFFUSE_PRECISION)]
+    # Diffuse inside predict() (K = N): an sc_gemm_precision to use at every N, or None for the
+    # N-based policy above.  The operator-level API (refinement.Diffuse) always uses split3.
+    self.diffuse_precision = None
     self.profile = None
 
   @classmethod
@@ -180,8 +177,6 @@ class Engine:
 
   # ---- operators (device in / device out)
   def gemm_engine(self, n: int) -> int:
-    if os.environ.get("SCB_FORCE_SIMT") == "1":    # debugging aid: validation GEMM everywhere
-      return nat.GEMM_SIMT
     return nat.GEMM_SIMT if n < self.simt_below else nat.GEMM_TCGEN05
 
   def affinity(self, x_dev, want_crop_vector: bool):
@@ -279,7 +274,7 @@ class Engine:
   @staticmethod
   def upper_pass_ok(sigma: float) -> bool:
     """The symmetric blur pair covers radius-4 filters (sigma ~ 1, every BASELINE config)."""
-    return sigma > 1e-15 and int(4.0 * sigma + 0.5) == 4 and os.environ.get("SCB_BLUR_TWO_PASS") != "1"
+    return sigma > 1e-15 and int(4.0 * sigma + 0.5) == 4
 
   def split_planes(self, a, n):
     hi, lo = self.planes(n)

@@ -548,13 +548,13 @@ def check_sharded_options(clusterer, num_embeddings: int):
     raise NotImplementedError("predict_sharded: single-cluster detection is not sharded")
   if clusterer.constraint_options:
     raise NotImplementedError("predict_sharded: constraints are not sharded")
+  from .spectral_clusterer import LANCZOS_MAX_PAIRS, lanczos_basis, lanczos_fits
   limit = clusterer.max_clusters + 1
-  if limit > 32:
+  if limit > LANCZOS_MAX_PAIRS:
     raise NotImplementedError("predict_sharded: max_clusters <= 31 (extremal eigensolver)")
-  basis = max(2 * limit + 32, 64)
-  if num_embeddings < 4 * basis:
+  if not lanczos_fits(num_embeddings, limit):
     raise ValueError("predict_sharded: n=%d is too small for the Lanczos basis (%d vectors); "
-                     "use predict()" % (num_embeddings, basis))
+                     "use predict()" % (num_embeddings, lanczos_basis(limit)))
 
 
 def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
@@ -637,16 +637,9 @@ def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
            None, w.ctypes.data_as(ctypes.c_void_p), dev._ptr(v),
            stats.ctypes.data_as(ctypes.c_void_p), eng.stream)
   descend = which == nat.EIG_LARGEST
-  if descend:
-    k, gap = utils.compute_number_of_clusters(
-        w, max_clusters=clusterer.max_clusters, stop_eigenvalue=clusterer.stop_eigenvalue,
-        eigengap_type=clusterer.eigengap_type, descend=True)
-  else:
-    if clusterer.eigengap_type == utils.EigenGapType.NormalizedDiff:
-      raise NotImplementedError("predict_sharded: NormalizedDiff on a Laplacian needs lambda_max")
-    k, gap = utils.compute_number_of_clusters(
-        w, max_clusters=clusterer.max_clusters, eigengap_type=clusterer.eigengap_type,
-        descend=False)
+  if not descend and clusterer.eigengap_type == utils.EigenGapType.NormalizedDiff:
+    raise NotImplementedError("predict_sharded: NormalizedDiff on a Laplacian needs lambda_max")
+  k, gap = clusterer._count_clusters(w, descend)
   clusterer.last_details = dict(eigenvalues=w.copy(), n_clusters_raw=k, max_gap=gap,
                                 solver="lanczos-sharded x%d" % world,
                                 transport=getattr(refiner, "last_transport", "local"),

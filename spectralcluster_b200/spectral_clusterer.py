@@ -37,6 +37,21 @@ RefinementOptions = refinement.RefinementOptions
 EigenGapType = utils.EigenGapType
 
 
+# The block Lanczos solver (sc_eigh_extremal) finds at most this many eigenpairs.
+LANCZOS_MAX_PAIRS = 32
+
+
+def lanczos_basis(limit: int) -> int:
+  """Basis vectors the block Lanczos solver is sized for when `limit` eigenpairs are wanted."""
+  return max(2 * limit + 32, 64)
+
+
+def lanczos_fits(n: int, limit: int) -> bool:
+  """Whether the block Lanczos solver takes `limit` eigenpairs of an n x n operator: it reads S a
+  handful of times but needs n >= 4 x its basis."""
+  return limit <= LANCZOS_MAX_PAIRS and n >= 4 * lanczos_basis(limit)
+
+
 class DeviceAffinity:
   """An affinity matrix resident in HBM (what predict() passes between its stages)."""
 
@@ -127,74 +142,51 @@ class SpectralClusterer:
     if self.max_clusters and self.max_clusters + 1 < limit:
       limit = self.max_clusters + 1
     n_vectors = min(n, max(limit, self.min_clusters or 0))
+    op = (refined.s, n, delta, left, right, sign)
+    counted = None          # (k, gap) when the solver already ran the eigengap
     if not refined.symmetric:
       # not symmetric nor diagonally similar to a symmetric matrix (e.g. RowWiseThreshold without
       # Symmetrize): np.linalg.eig + .real semantics (utils.py:59-61) by Krylov-Schur
       from . import arnoldi
-      w, v, stats = arnoldi.eig_extremal_device(eng, refined.s, n, delta, left, right, sign,
-                                                not descend, limit, n_vectors)
-      if descend:
-        k, gap = utils.compute_number_of_clusters(
-            w, max_clusters=self.max_clusters, stop_eigenvalue=self.stop_eigenvalue,
-            eigengap_type=self.eigengap_type, descend=True)
+      solver = "krylov-schur"
+      w, v, stats = arnoldi.eig_extremal_device(eng, *op, not descend, limit, n_vectors)
+      top_solve = lambda: arnoldi.eig_extremal_device(eng, *op, False, 1, 0)[0]
+    elif n > eng.dense_eig_max and lanczos_fits(n, limit):
+      solver = "lanczos"
+      w, v, stats = eng.eigh(*op, which, limit, n_vectors, False)
+      stats = stats.tolist()
+      top_solve = lambda: eng.eigh(*op, nat.EIG_LARGEST, 1, 0, False)[0]
+    else:
+      # the dense solver (Householder tridiagonalisation, 4/3 n^3): small matrices, and
+      # max_clusters=None / > 31 (every eigenvalue, or more pairs than Lanczos finds, is needed)
+      solver, stats, top_solve = "dense", None, None
+      if limit == n and n > 256:
+        # every eigenvalue is needed (max_clusters=None scans the whole spectrum, utils.py:100-102)
+        # but only the columns predict() will select: the eigengap runs between the two phases
+        def picker(values):
+          nonlocal counted
+          counted = self._count_clusters(values, descend)
+          return max(counted[0], self.min_clusters or 0, 1)
+
+        w, v = eng.eigh_dense_pick(*op, which, picker)
       else:
-        if self.eigengap_type == EigenGapType.NormalizedDiff and limit < n:
-          top, _, _ = arnoldi.eig_extremal_device(eng, refined.s, n, delta, left, right, sign,
-                                                  False, 1, 0)
-          w = np.concatenate([w, top])
-        k, gap = utils.compute_number_of_clusters(
-            w, max_clusters=self.max_clusters, eigengap_type=self.eigengap_type, descend=False)
-      self.last_details = dict(eigenvalues=np.array(w[:limit]), n_clusters_raw=k, max_gap=gap,
-                               solver="krylov-schur", lanczos_stats=stats)
-      return w, v, k, gap
-    # The block Lanczos solver needs n >= 4 max(2*limit+32, 64) and reads S a handful of times; the
-    # dense solver (Householder tridiagonalisation, 4/3 n^3) is kept for small matrices and for
-    # max_clusters=None / > 31 (every eigenvalue, or more than the extremal solver's 32, is needed).
-    basis = max(2 * limit + 32, 64)
-    dense = (n <= eng.dense_eig_max or n < 4 * basis or not self.max_clusters or limit > 32)
-
-    def count_clusters(values):
-      if descend:
-        return utils.compute_number_of_clusters(
-            values, max_clusters=self.max_clusters, stop_eigenvalue=self.stop_eigenvalue,
-            eigengap_type=self.eigengap_type, descend=True)
-      return utils.compute_number_of_clusters(
-          values, max_clusters=self.max_clusters, eigengap_type=self.eigengap_type, descend=False)
-
-    if dense and limit == n and n > 256:
-      # every eigenvalue is needed (max_clusters=None scans the whole spectrum, utils.py:100-102)
-      # but only the columns predict() will select: the eigengap runs between the two phases
-      picked = {}
-
-      def picker(values):
-        picked["k"], picked["gap"] = count_clusters(values)
-        return max(picked["k"], self.min_clusters or 0, 1)
-
-      w, v = eng.eigh_dense_pick(refined.s, n, delta, left, right, sign, which, picker)
-      k, gap = picked["k"], picked["gap"]
-      self.last_details = dict(eigenvalues=np.array(w[:limit]), n_clusters_raw=k, max_gap=gap,
-                               solver="dense", lanczos_stats=None)
-      return w, v, k, gap
-    if dense:
-      w, v, stats = eng.eigh(refined.s, n, delta, left, right, sign, which, n, n_vectors, True)
-    else:
-      w, v, stats = eng.eigh(refined.s, n, delta, left, right, sign, which, limit, n_vectors,
-                             False)
-      if not descend and self.eigengap_type == EigenGapType.NormalizedDiff:
-        # np.max(eigenvalues) of the full spectrum (utils.py:109): one more extremal solve
-        top, _, _ = eng.eigh(refined.s, n, delta, left, right, sign, nat.EIG_LARGEST, 1, 0, False)
-        w = np.concatenate([w, top])
-    if descend:
-      k, gap = utils.compute_number_of_clusters(
-          w, max_clusters=self.max_clusters, stop_eigenvalue=self.stop_eigenvalue,
-          eigengap_type=self.eigengap_type, descend=True)
-    else:
-      k, gap = utils.compute_number_of_clusters(
-          w, max_clusters=self.max_clusters, eigengap_type=self.eigengap_type, descend=False)
+        w, v, _ = eng.eigh(*op, which, n, n_vectors, True)
+    if (top_solve is not None and limit < n and not descend and
+        self.eigengap_type == EigenGapType.NormalizedDiff):
+      # np.max(eigenvalues) of the full spectrum (utils.py:109): one more extremal solve
+      w = np.concatenate([w, top_solve()])
+    k, gap = counted or self._count_clusters(w, descend)
     self.last_details = dict(eigenvalues=np.array(w[:limit]), n_clusters_raw=k, max_gap=gap,
-                             solver="dense" if dense else "lanczos",
-                             lanczos_stats=None if dense else stats.tolist())
+                             solver=solver, lanczos_stats=stats)
     return w, v, k, gap
+
+  def _count_clusters(self, eigenvalues, descend: bool):
+    """utils.compute_number_of_clusters with this clusterer's options -> (k, max gap); only a
+    descending spectrum stops at stop_eigenvalue."""
+    stop = dict(stop_eigenvalue=self.stop_eigenvalue) if descend else {}
+    return utils.compute_number_of_clusters(eigenvalues, max_clusters=self.max_clusters,
+                                            eigengap_type=self.eigengap_type, descend=descend,
+                                            **stop)
 
   def _compute_eigenvectors_ncluster(self, affinity, constraint_matrix=None):
     """(eigenvectors, n_clusters, max eigengap) for an affinity matrix.

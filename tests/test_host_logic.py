@@ -98,7 +98,30 @@ class FakeEngine:
 
   def row_stats(self, a, n, want_max=True, want_sum=True):
     self._rec("row_stats", want_max, want_sum)
-    return (torch.ones(self.n, dtype=torch.float64) * 2.0, None)
+    return (torch.ones(self.n, dtype=torch.float64) * 2.0,
+            torch.ones(self.n, dtype=torch.float64) * 3.0 if want_sum else None)
+
+  # ---- eigen stage: which solver runs, with which arguments
+  dense_eig_max = 0
+
+  def diffuse_precision_for(self, n):
+    return None
+
+  @staticmethod
+  def _spectrum(count, which):
+    # a clear gap after the third value, in the order the solver returns them
+    w = np.array([5.0, 4.0, 3.0] + [0.5 * 0.999 ** i for i in range(max(count - 3, 0))])[:count]
+    return w if which == nat.EIG_LARGEST else 5.0 - w
+
+  def eigh(self, s, n, delta, left, right, sign, which, n_values, n_vectors, dense, tol=1e-9,
+           max_matvecs=0):
+    self._rec("eigh", which, n_values, n_vectors, dense)
+    return self._spectrum(n_values, which), "V", np.zeros(4, dtype=np.int64)
+
+  def eigh_dense_pick(self, s, n, delta, left, right, sign, which, picker):
+    w = self._spectrum(n, which)
+    self._rec("eigh_dense_pick", which, picker(w))
+    return w, "V"
 
 
 def names(eng):
@@ -157,3 +180,63 @@ def test_planner_variants():
   assert names(eng) == ["row_normalize", "diffuse"] and out.symmetric
   with pytest.raises(ValueError):
     dev.run_refinement(FakeEngine(10), "A", 10, scb.RefinementOptions(refinement_sequence=["x"]))
+
+
+L, S = nat.EIG_LARGEST, nat.EIG_SMALLEST
+UNNORM = scb.LaplacianType.Unnormalized
+RATIO, NDIFF = scb.EigenGapType.Ratio, scb.EigenGapType.NormalizedDiff
+
+
+# (n, max_clusters, min_clusters, laplacian, eigengap, symmetric, dense_eig_max) ->
+# (solver calls in order, last_details["solver"]).  max_clusters = 10: the Lanczos basis is 64
+# vectors, so Lanczos needs n >= 256; max_clusters = 31: basis 96, n >= 384.
+@pytest.mark.parametrize("case,calls,solver", [
+    ((2000, 10, None, None, RATIO, True, 0), [("eigh", L, 11, 11, False)], "lanczos"),
+    ((256, 10, None, None, RATIO, True, 0), [("eigh", L, 11, 11, False)], "lanczos"),
+    ((255, 10, None, None, RATIO, True, 0), [("eigh", L, 255, 11, True)], "dense"),
+    ((2000, 10, 15, None, RATIO, True, 0), [("eigh", L, 11, 15, False)], "lanczos"),
+    ((2000, 10, None, None, RATIO, True, 2000), [("eigh", L, 2000, 11, True)], "dense"),
+    ((2000, 31, None, None, RATIO, True, 0), [("eigh", L, 32, 32, False)], "lanczos"),
+    ((383, 31, None, None, RATIO, True, 0), [("eigh", L, 383, 32, True)], "dense"),
+    ((2000, 32, None, None, RATIO, True, 0), [("eigh", L, 2000, 33, True)], "dense"),
+    ((2000, None, None, None, RATIO, True, 0), [("eigh_dense_pick", L, 3)], "dense"),
+    ((2000, None, 5, UNNORM, RATIO, True, 0), [("eigh_dense_pick", S, 5)], "dense"),
+    ((200, None, None, None, RATIO, True, 0), [("eigh", L, 200, 200, True)], "dense"),
+    ((2000, 10, None, UNNORM, RATIO, True, 0), [("eigh", S, 11, 11, False)], "lanczos"),
+    ((2000, 10, None, UNNORM, NDIFF, True, 0),
+     [("eigh", S, 11, 11, False), ("eigh", L, 1, 0, False)], "lanczos"),
+    ((2000, 10, None, None, NDIFF, True, 0), [("eigh", L, 11, 11, False)], "lanczos"),
+    ((200, 10, None, UNNORM, NDIFF, True, 0), [("eigh", S, 200, 11, True)], "dense"),
+    ((2000, None, None, UNNORM, NDIFF, True, 0), [("eigh_dense_pick", S, 3)], "dense"),
+    ((2000, 10, None, None, RATIO, False, 0), [("arnoldi", False, 11, 11)], "krylov-schur"),
+    ((2000, 10, 15, None, NDIFF, False, 0), [("arnoldi", False, 11, 15)], "krylov-schur"),
+    ((2000, 10, None, UNNORM, RATIO, False, 0), [("arnoldi", True, 11, 11)], "krylov-schur"),
+    ((2000, 10, None, UNNORM, NDIFF, False, 0),
+     [("arnoldi", True, 11, 11), ("arnoldi", False, 1, 0)], "krylov-schur"),
+    ((200, None, None, UNNORM, NDIFF, False, 0), [("arnoldi", True, 200, 200)], "krylov-schur"),
+])
+def test_eigen_stage_solver_choice(monkeypatch, case, calls, solver):
+  """Which eigensolver _eigen_on_device() runs, with which arguments, and whether it adds the
+  lambda_max solve NormalizedDiff needs on an ascending spectrum."""
+  from spectralcluster_b200 import arnoldi
+  n, max_clusters, min_clusters, laplacian, eigengap, symmetric, dense_eig_max = case
+  eng = FakeEngine(n)
+  eng.dense_eig_max = dense_eig_max
+
+  def fake_arnoldi(eng_, s, n_, delta, left, right, sign, smallest, n_values, n_vectors):
+    eng_._rec("arnoldi", smallest, n_values, n_vectors)
+    return FakeEngine._spectrum(n_values, S if smallest else L), "V", [0, 0, 0, 0]
+
+  monkeypatch.setattr(arnoldi, "eig_extremal_device", fake_arnoldi)
+  sc = scb.SpectralClusterer(min_clusters=min_clusters, max_clusters=max_clusters,
+                             laplacian_type=laplacian, eigengap_type=eigengap)
+  w, v, k, gap = sc._eigen_on_device(eng, scb.spectral_clusterer.DeviceAffinity("A", n, None,
+                                                                                 symmetric))
+  solves = [c for c in eng.calls if c[0] != "row_stats"]
+  assert solves == calls
+  assert v == "V" and k == 3
+  assert sc.last_details["solver"] == solver
+  assert sc.last_details["n_clusters_raw"] == k and sc.last_details["max_gap"] == gap
+  limit = n if not max_clusters else min(n, max_clusters + 1)
+  assert len(sc.last_details["eigenvalues"]) == min(limit, len(w))
+  assert (sc.last_details["lanczos_stats"] is None) == (solver == "dense")

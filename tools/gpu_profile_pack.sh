@@ -15,7 +15,7 @@ timeout 600 $NCU --metrics gpu__time_duration.sum --csv --log-file $out/${tag}_l
 python tools/summarize_launches.py $out/${tag}_launches_n${n}.csv > $out/${tag}_launches_n${n}.txt 2>&1
 
 # 2. full captures: refinement pair, both GEMMs, the block matvec
-timeout 900 $NCU --set full --import-source on -k regex:'k_blur_band|k_thrsym_upper|k_gemm_wgmma|k_symm_dmma|k_symm_f32_f64|k_block_proj' \
+timeout 900 $NCU --set full --import-source on -k regex:'k_blur_band|k_thrsym_upper|k_gemm_wgmma|k_symm_dmma|k_block_proj' \
   -c 7 -o $out/${tag}_full_n${n} -f python tools/profile_step.py --n $n > $out/${tag}_full_n${n}.log 2>&1
 python tools/ncu_summary.py $out/${tag}_full_n${n}.ncu-rep > $out/${tag}_ncu_full_n${n}.txt 2>&1
 

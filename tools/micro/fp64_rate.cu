@@ -1,6 +1,6 @@
 // Micro-benchmark: fp64 FMA throughput of sm_90a through the CUDA cores (DFMA) and through the
-// tensor cores (mma.sync.m8n8k4.f64 -> DMMA), to decide which one the Lanczos block product
-// (eigh_lanczos.cu, k_symm_f32_f64) should be built on.
+// tensor cores (mma.sync.m8n8k4.f64 -> DMMA): the comparison behind building the Lanczos block
+// product (eigh_lanczos.cu, k_symm_dmma) on DMMA.
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_rate tools/micro/fp64_rate.cu && ./fp64_rate
 #include <cstdio>
 #include <cuda_runtime.h>
