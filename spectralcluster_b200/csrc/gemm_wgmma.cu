@@ -11,13 +11,13 @@
 // missing Ahi*Blo term is a zero-mean 2^-12 relative perturbation per product that averages down
 // with sqrt(K)); SC_GEMM_SINGLE issues only hi*hi (2^-11 on both sides).
 //
-// Structure (one CTA per SM, persistent, 384 threads = 3 warpgroups, 128 x 128 output tile):
+// Structure (one CTA per SM, persistent, 384 threads = 3 warpgroups, 128 x BN output tile):
 //   warpgroup 0  warp 0 lane 0 is the TMA producer: cp.async.bulk.tensor.2d (SWIZZLE_128B) of the
 //                4 (or 3, 2) planes of a K block into a ring of stages, completion on an mbarrier
 //                (expect_tx); paced against the other CTAs' producers through a global
 //                checkpoint counter (see below)
 //   warpgroups 1-2  consumers (setmaxnreg 232): each owns 64 rows of the tile and issues
-//                wgmma.m64n128k16 from shared-memory descriptors into a register chain
+//                wgmma.m64n{BN}k16 from shared-memory descriptors into a register chain
 //                accumulator.  A chain is only CHUNK_KB K-blocks long; at its end the chain is
 //                added, round-to-nearest, into a second register tile (the tensor core's fp32
 //                accumulation truncates, so long chains drift low -- the two-level scheme keeps the
@@ -25,9 +25,15 @@
 //                straight from registers: (x+1)/2 + off-diagonal row maximum (affinity), row
 //                maximum / sum (Diffuse), the stores, and the mirrored (transposed) stores of the
 //                symmetric variant.
+// Tile width BN: the Diffuse products at one or two MMAs (EPI_PLAIN, SINGLE / SPLIT2) use
+// 128 x 192 tiles.  Each consumer warpgroup reads its A half and all of B from shared memory per
+// wgmma, so the wider tile moves ~14 % fewer shared-memory bytes and 17 % fewer L2 bytes per MMA;
+// the chain and sum accumulators (96 + 96 registers per thread) still fit the 232 of setmaxnreg.
+// SPLIT3 keeps 128 x 128 (at 192 its 72 KB stages would leave a ring of 2), and so does the
+// affinity (K = d: bound by its stores, not by operand traffic).
 // Tiles are rasterised in groups of 16 M-blocks so that a wave of CTAs shares 16 A-panels and ~8
-// B-panels through L2; the symmetric variant (C = Y Y^T) computes only the tiles on and above the
-// diagonal.
+// B-panels through L2.  The symmetric variant (C = Y Y^T) computes only the tiles that reach the
+// upper triangle, tile (m, n) iff BN n + BN - 1 >= BM m, and stores the mirrored half from them.
 #include "common.cuh"
 
 #include <cuda.h>
@@ -37,11 +43,10 @@
 
 namespace sc {
 
-constexpr int BM = 128, BN = 128, BK = 64;          // BK fp16 = 128 bytes = one swizzle row
+constexpr int BM = 128, BK = 64;                     // BK fp16 = 128 bytes = one swizzle row
 constexpr int WG_M = 64;                             // rows of the tile per consumer warpgroup
 constexpr int MMA_K = 16;
 constexpr int A_PLANE_BYTES = BM * BK * 2;           // 16 KB
-constexpr int B_PLANE_BYTES = BN * BK * 2;           // 16 KB
 constexpr int GROUP_M = 16;
 // K-blocks between pacing checkpoints of the producers.  The window the CTAs of a wave may drift
 // apart is PACE_KB x ~0.4-0.8 MB of operand panels per K block; 32 keeps it well inside L2.
@@ -54,7 +59,6 @@ constexpr int NUM_CONSUMER_WARPS = 8;
 constexpr int NUM_THREADS = 128 + NUM_CONSUMER_WARPS * 32;   // 384
 
 static_assert(BM == 2 * WG_M, "two consumer warpgroups of 64 rows each");
-static_assert(BM == BN, "the symmetric tile enumeration assumes square tiles");
 
 enum { TC_EPI_PLAIN = 0, TC_EPI_AFFINITY = 1 };
 
@@ -122,32 +126,65 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   return d;
 }
 
-// D[64 x 128] (+)= A[64 x 16] B[128 x 16]^T, fp16 in, fp32 accumulate; scale_d = 0 overwrites D.
+// D[64 x BN] (+)= A[64 x 16] B[BN x 16]^T, fp16 in, fp32 accumulate; scale_d = 0 overwrites D.
 // Fragment of thread t of the warpgroup: warp w = t / 32, lane l; d[4 j + 2 h + e] is row
-// 16 w + l / 4 + 8 h, column 8 j + 2 (l % 4) + e.
-__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc,
-                                                 uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-      "%64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
-        "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),
-        "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),
-        "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),
-        "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]),
-        "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]),
-        "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]),
-        "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]),
-        "+f"(d[62]), "+f"(d[63])
-      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+// 16 w + l / 4 + 8 h, column 8 j + 2 (l % 4) + e, j < BN / 8.
+template <int BN>
+__device__ __forceinline__ void wgmma_m64k16(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc,
+                                             uint32_t scale_d) {
+  static_assert(BN == 128 || BN == 192, "wgmma tile width");
+  if constexpr (BN == 128) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]),
+          "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+          "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]),
+          "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+          "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+          "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d));
+  } else {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %98, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n192k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+        "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
+        "%96, %97, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),
+          "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]),
+          "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+          "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+          "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]),
+          "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+          "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+          "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]),
+          "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]),
+          "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]),
+          "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]),
+          "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]),
+          "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d));
+  }
 }
 
 struct TileCoord {
@@ -155,9 +192,10 @@ struct TileCoord {
 };
 
 // Rasterisation.  Full problem: groups of GROUP_M M-blocks sweep all N-blocks.  Symmetric
-// problem (C = Y Y^T): only tiles on or above the diagonal are computed, i.e. m_blk <= n_blk;
-// the rest is filled by mirrored stores.  group_start[g] is the first tile index of group g
-// (host-computed with the same counting rule).
+// problem (C = Y Y^T): only the tiles that reach the upper triangle (c >= r) are computed, i.e.
+// tile (m, n) iff its last column BN n + BN - 1 >= its first row BM m; the rest is filled by
+// mirrored stores.  group_start[g] is the first tile index of group g (host-computed with the
+// same counting rule).  Any BN works here; BN is a multiple of 8 for the epilogue fragments.
 constexpr int MAX_GROUPS = 160;
 struct TileTable {
   int group_start[MAX_GROUPS + 1];
@@ -165,20 +203,27 @@ struct TileTable {
   int num_tiles;
 };
 
+template <int BN>
 __host__ __device__ inline int sym_valid_mblocks(int g, int n_blk, int tiles_m) {
-  // m blocks of group g that are valid for column block n_blk: m_blk <= n_blk
-  int lim = n_blk + 1 - g * GROUP_M;
+  // m blocks of group g that are valid for column block n_blk: BM m_blk <= BN n_blk + BN - 1
+  int lim = (n_blk * BN + BN - 1) / BM + 1 - g * GROUP_M;
   const int avail = tiles_m - g * GROUP_M;
   if (lim > GROUP_M) lim = GROUP_M;
   if (lim > avail) lim = avail;
   return lim < 0 ? 0 : lim;
 }
 
+// first column block whose tiles reach the first row of group g
+template <int BN>
+__host__ __device__ inline int sym_first_nblk(int g) {
+  return g * GROUP_M * BM / BN;
+}
+
 // Tile coordinates for a CTA that walks tile, tile + stride, tile + 2 stride, ...: the symmetric
 // table search would cost ~1 k instructions per call, which is noise at K = N but not at K = d
 // (affinity), so the cursor moves forward inside the (group, column block) enumeration instead
 // of restarting it.
-template <bool SYM>
+template <bool SYM, int BN>
 struct TileCursor {
   int tiles_m, tiles_n;
   int g, nb, base;          // SYM: current group, column block, first tile index of (g, nb)
@@ -199,11 +244,11 @@ struct TileCursor {
       // tiles are visited in increasing order: move forward only
       while (g + 1 < tab.num_groups && tab.group_start[g + 1] <= tile) {
         ++g;
-        nb = g * GROUP_M;              // first column block that touches the group
+        nb = sym_first_nblk<BN>(g);
         base = tab.group_start[g];
       }
       for (;;) {
-        const int cnt = sym_valid_mblocks(g, nb, tiles_m);
+        const int cnt = sym_valid_mblocks<BN>(g, nb, tiles_m);
         if (tile - base < cnt) break;
         base += cnt;
         ++nb;
@@ -215,16 +260,18 @@ struct TileCursor {
   }
 };
 
-template <int PREC>
+template <int PREC, int BN>
 struct StageGeom {
-  // planes of one K block in a stage: [A_hi][B_hi][A_lo (PREC>=2)][B_lo (PREC==3)]
+  // planes of one K block in a stage: [A_hi][B_hi][A_lo (PREC>=2)][B_lo (PREC==3)], each a
+  // multiple of the 1 KB swizzle atom.  BN = 192: 40 KB x 5 stages (single), 56 KB x 4 (split2).
+  static constexpr int B_PLANE_BYTES = BN * BK * 2;
   static constexpr int BYTES =
       A_PLANE_BYTES * (PREC >= 2 ? 2 : 1) + B_PLANE_BYTES * (PREC == 3 ? 2 : 1);
   static constexpr int BUDGET = 227 * 1024 - 1024 - 256;
   static constexpr int STAGES = (BUDGET / BYTES) > 8 ? 8 : (BUDGET / BYTES);
 };
 
-template <int PREC, int EPI, bool SYM>
+template <int PREC, int EPI, bool SYM, int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
              const __grid_constant__ CUtensorMap map_a_lo,
@@ -235,8 +282,13 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
              int diag_shift, unsigned int* __restrict__ pace, int pace_kb,
              float* __restrict__ stat_rowmax, double* __restrict__ stat_rowsum,
              float* __restrict__ mirror_out, int64_t ldm, int aff_chunk_kb) {
-  constexpr int STAGES = StageGeom<PREC>::STAGES;
-  constexpr int STAGE_BYTES = StageGeom<PREC>::BYTES;
+  constexpr int STAGES = StageGeom<PREC, BN>::STAGES;
+  constexpr int STAGE_BYTES = StageGeom<PREC, BN>::BYTES;
+  constexpr int B_PLANE_BYTES = StageGeom<PREC, BN>::B_PLANE_BYTES;
+  constexpr int NACC = BN / 2;          // accumulator registers per thread and tile
+  // The affinity stores its diagonal tiles whole, without the mask of the straddling tiles below:
+  // that needs square tiles.
+  static_assert(EPI == TC_EPI_PLAIN || BN == BM, "the affinity runs on square tiles");
   // K blocks per register chain.  Diffuse: 2 (split) / 4 (single).  Affinity (K = d):
   // `aff_chunk_kb` from the host, 1 by default -- the affinity feeds a threshold, so it gets the
   // shortest chains (SCB_AFFINITY_CHUNK_KB overrides).
@@ -282,7 +334,7 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
       // bounded, it is only a hint -- until the whole grid has reached the same checkpoint.
       const int ck_per_tile = (num_kb + pace_kb - 1) / pace_kb;
       unsigned int passed = 0;
-      TileCursor<SYM> cursor;
+      TileCursor<SYM, BN> cursor;
       cursor.init(tiles_m, tiles_n);
       for (int round = 0; round * (int)gridDim.x < num_tiles; ++round) {
         const int tile = round * (int)gridDim.x + (int)blockIdx.x;
@@ -325,15 +377,15 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
   const int wq = warp & 3;                              // rows [16 wq, +16) of those
   int stage = 0;
   uint32_t phase = 0;
-  float acc[64], sum[64];
+  float acc[NACC], sum[NACC];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
-  TileCursor<SYM> cursor;
+  for (int i = 0; i < NACC; ++i) acc[i] = 0.0f;
+  TileCursor<SYM, BN> cursor;
   cursor.init(tiles_m, tiles_n);
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
     const TileCoord tc = cursor.at(tile, tab);
 #pragma unroll
-    for (int i = 0; i < 64; ++i) sum[i] = 0.0f;
+    for (int i = 0; i < NACC; ++i) sum[i] = 0.0f;
     // One chain per pass of the outer loop.  Its end is a structural wait<0>, so the compiler sees
     // no path on which accumulator registers are read while a wgmma group is in flight (a wait
     // on a data-dependent branch makes ptxas drain the pipe at every K block).
@@ -357,20 +409,20 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
 #pragma unroll
           for (int kk = 0; kk < BK / MMA_K; ++kk) {
             const uint64_t adv = (uint64_t)(kk * MMA_K * 2 / 16);
-            wgmma_m64n128k16(acc, a_hi + adv, b_lo + adv, (in_chunk | kk) ? 1u : 0u);
-            wgmma_m64n128k16(acc, a_lo + adv, b_hi + adv, 1u);
+            wgmma_m64k16<BN>(acc, a_hi + adv, b_lo + adv, (in_chunk | kk) ? 1u : 0u);
+            wgmma_m64k16<BN>(acc, a_lo + adv, b_hi + adv, 1u);
           }
         } else if (PREC == 2) {
 #pragma unroll
           for (int kk = 0; kk < BK / MMA_K; ++kk) {
             const uint64_t adv = (uint64_t)(kk * MMA_K * 2 / 16);
-            wgmma_m64n128k16(acc, a_lo + adv, b_hi + adv, (in_chunk | kk) ? 1u : 0u);
+            wgmma_m64k16<BN>(acc, a_lo + adv, b_hi + adv, (in_chunk | kk) ? 1u : 0u);
           }
         }
 #pragma unroll
         for (int kk = 0; kk < BK / MMA_K; ++kk) {
           const uint64_t adv = (uint64_t)(kk * MMA_K * 2 / 16);
-          wgmma_m64n128k16(acc, a_hi + adv, b_hi + adv, (PREC >= 2 || in_chunk || kk) ? 1u : 0u);
+          wgmma_m64k16<BN>(acc, a_hi + adv, b_hi + adv, (PREC >= 2 || in_chunk || kk) ? 1u : 0u);
         }
         wgmma_commit();
         // one group in flight: the previous K block's buffer is free once this one is queued
@@ -383,21 +435,29 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
       wgmma_wait<0>();
       if (lane == 0) mbar_arrive(smem_u32(&empty_bar[pending]));
 #pragma unroll
-      for (int i = 0; i < 64; ++i) sum[i] += acc[i];
+      for (int i = 0; i < NACC; ++i) sum[i] += acc[i];
     }
 
     // ---- epilogue, straight from the accumulator fragment: this thread holds rows r0 and r0 + 8
-    // of the tile, columns 8 j + 2 (lane % 4) + {0, 1} for j = 0..15.
+    // of the tile, columns 8 j + 2 (lane % 4) + {0, 1} for j < BN / 8.
     const int64_t r0 = (int64_t)tc.m_blk * BM + wg * WG_M + wq * 16 + (lane >> 2);
     const int64_t col0 = (int64_t)tc.n_blk * BN + 2 * (lane & 3);
     const int64_t tile_row0 = (int64_t)tc.m_blk * BM, tile_col0 = (int64_t)tc.n_blk * BN;
     const bool full = (tile_row0 + BM <= M) && (tile_col0 + BN <= N);     // CTA-uniform
-    // the tiles below the diagonal are skipped: every tile strictly above it also stores its
-    // transpose
-    const bool mirror = SYM && tc.n_blk > tc.m_blk;
+    // Symmetric product: the tiles below the diagonal are skipped; every tile wholly above it also
+    // stores its transpose.  A Diffuse tile that straddles the diagonal stores element (r, c) iff
+    // c >= r and its mirror (c, r) iff c > r, so each element of C is written once, from one
+    // accumulator, and C is bitwise symmetric; its row statistics take c >= r, the mirrored
+    // column statistics r < c.  The affinity's square diagonal tiles store every element directly.
+    // Both flags are CTA-uniform: the tiles wholly above the diagonal run unmasked.
+    const bool above = SYM && tile_col0 >= tile_row0 + BM;
+    const bool straddle = SYM && EPI == TC_EPI_PLAIN && !above;
+    const bool mirror = above || straddle;
+    // in a straddling tile, element (r0 + 8 h, col0 + x) lies on the diagonal iff x = diag + 8 h
+    const int diag = (int)(r0 - col0);
     if (EPI == TC_EPI_AFFINITY) {
 #pragma unroll
-      for (int i = 0; i < 64; ++i) sum[i] = fmaf(sum[i], 0.5f, 0.5f);   // (x + 1) / 2, utils.py:39
+      for (int i = 0; i < NACC; ++i) sum[i] = fmaf(sum[i], 0.5f, 0.5f);   // (x + 1) / 2, utils.py:39
     }
     const bool row_stats = (EPI == TC_EPI_AFFINITY && rowmax_offdiag != nullptr) ||
                            (EPI == TC_EPI_PLAIN && stat_rowmax != nullptr);
@@ -408,7 +468,7 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
         const int64_t dcol = row + diag_shift;          // this row's diagonal column (affinity)
         float mx = 0.0f, sm = 0.0f;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
+        for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int64_t col = col0 + 8 * j + e;
@@ -417,7 +477,7 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
             // non-negative maximum; affinity: 0.5, excluded)
             if (EPI == TC_EPI_AFFINITY) {
               if (col != dcol && (full || col < N)) mx = fmaxf(mx, v);
-            } else {
+            } else if (!straddle || 8 * j + e >= diag + 8 * h) {
               mx = fmaxf(mx, v);
               sm += v;
             }
@@ -443,13 +503,14 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
       // the mirrored elements of column c form a piece of ROW c of C: column reductions over the
       // tile's rows (rows past M are skipped)
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
+      for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
+          const int64_t tr = col0 + 8 * j + e;
           float mx = 0.0f, sm = 0.0f;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            if (full || r0 + 8 * h < M) {
+            if ((full || r0 + 8 * h < M) && (!straddle || 8 * j + e > diag + 8 * h)) {
               const float v = sum[4 * j + 2 * h + e];
               mx = fmaxf(mx, v);
               sm += v;
@@ -460,7 +521,6 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
             if (EPI == TC_EPI_PLAIN) sm += __shfl_xor_sync(0xffffffffu, sm, o);
           }
-          const int64_t tr = col0 + 8 * j + e;
           if (lane < 4 && tr < N) {
             if (EPI == TC_EPI_AFFINITY) {
               atomic_max_nonneg(rowmax_offdiag + tr, mx);
@@ -479,9 +539,11 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
       if (!full && row >= M) continue;
       float* dst = C + row * ldc + col0;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
+      for (int j = 0; j < BN / 8; ++j) {
         const float2 v = make_float2(sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
-        if (full || col0 + 8 * j + 1 < N) {
+        if (straddle && 8 * j < diag + 8 * h) {          // c < r comes from the mirror of (c, r)
+          if (8 * j + 1 == diag + 8 * h) dst[8 * j + 1] = v.y;
+        } else if (full || col0 + 8 * j + 1 < N) {
           *reinterpret_cast<float2*>(dst + 8 * j) = v;
         } else if (col0 + 8 * j < N) {
           dst[8 * j] = v.x;
@@ -500,11 +562,12 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
         const int64_t row = r0 + 8 * h;
         if (!full && row >= M) continue;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
+        for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int64_t col = col0 + 8 * j + e;
-            if (full || col < N) tdst[col * ldt + row] = sum[4 * j + 2 * h + e];
+            if ((full || col < N) && (!straddle || 8 * j + e > diag + 8 * h))
+              tdst[col * ldt + row] = sum[4 * j + 2 * h + e];
           }
         }
       }
@@ -550,28 +613,43 @@ static int make_plane_map(CUtensorMap* map, const __half* ptr, int64_t rows, int
   return 0;
 }
 
+template <int BN>
 static void build_tile_table(TileTable& tab, int tiles_m, int tiles_n) {
   tab.num_groups = (tiles_m + GROUP_M - 1) / GROUP_M;
   int total = 0;
   for (int g = 0; g < tab.num_groups; ++g) {
     tab.group_start[g] = total;
-    for (int nb = g * GROUP_M; nb < tiles_n; ++nb) total += sym_valid_mblocks(g, nb, tiles_m);
+    for (int nb = sym_first_nblk<BN>(g); nb < tiles_n; ++nb)
+      total += sym_valid_mblocks<BN>(g, nb, tiles_m);
   }
   tab.group_start[tab.num_groups] = total;
   tab.num_tiles = total;
 }
 
-template <int PREC, int EPI, bool SYM>
-static int launch(const sc_context* ctx, const CUtensorMap& ah, const CUtensorMap& al,
-                  const CUtensorMap& bh, const CUtensorMap& bl, int M, int N, int K, float* C,
-                  int64_t ldc, float* rowmax, int diag_shift, float* stat_rowmax,
+template <int PREC, int EPI, bool SYM, int BN>
+static int launch(const sc_context* ctx, const __half* a_hi, const __half* a_lo, int64_t lda,
+                  const __half* b_hi, const __half* b_lo, int64_t ldb, int M, int N, int K,
+                  float* C, int64_t ldc, float* rowmax, int diag_shift, float* stat_rowmax,
                   double* stat_rowsum, float* mirror, int64_t ldm, cudaStream_t st) {
-  constexpr int STAGES = StageGeom<PREC>::STAGES;
-  constexpr int STAGE_BYTES = StageGeom<PREC>::BYTES;
+  constexpr int STAGES = StageGeom<PREC, BN>::STAGES;
+  constexpr int STAGE_BYTES = StageGeom<PREC, BN>::BYTES;
   static_assert(STAGES >= 2, "wgmma GEMM: the operand ring needs at least two stages");
+  CUtensorMap ah, al, bh, bl;
+  if (int r = make_plane_map(&ah, a_hi, M, K, lda, BM)) return r;
+  if (int r = make_plane_map(&bh, b_hi, N, K, ldb, BN)) return r;
+  al = ah;
+  bl = bh;
+  if (PREC >= 2) {
+    SC_REQUIRE(a_lo, "wgmma GEMM: the lo plane of A is missing");
+    if (int r = make_plane_map(&al, a_lo, M, K, lda, BM)) return r;
+  }
+  if (PREC == 3) {
+    SC_REQUIRE(b_lo, "wgmma GEMM: the lo plane of B is missing");
+    if (int r = make_plane_map(&bl, b_lo, N, K, ldb, BN)) return r;
+  }
   const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
   SC_REQUIRE(smem <= ctx->smem_optin, "wgmma GEMM needs %zu B of shared memory", smem);
-  auto kern = k_gemm_wgmma<PREC, EPI, SYM>;
+  auto kern = k_gemm_wgmma<PREC, EPI, SYM, BN>;
   SC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
   TileTable tab = {};
@@ -579,7 +657,7 @@ static int launch(const sc_context* ctx, const CUtensorMap& ah, const CUtensorMa
   if (SYM) {
     SC_REQUIRE((tiles_m + GROUP_M - 1) / GROUP_M <= MAX_GROUPS, "wgmma GEMM: N too large for "
                "the symmetric tile table");
-    build_tile_table(tab, tiles_m, tiles_n);
+    build_tile_table<BN>(tab, tiles_m, tiles_n);
     tiles = tab.num_tiles;
   }
   int sms = ctx->sm_count;
@@ -622,38 +700,29 @@ int gemm_nt_wgmma(const sc_context* ctx, int epi, int precision, const __half* a
              precision == SC_GEMM_SINGLE, "wgmma GEMM: unknown precision %d", precision);
   SC_REQUIRE((stat_rowmax == nullptr) == (stat_rowsum == nullptr),
              "wgmma GEMM: the row statistics come together");
-  const int prec = precision == SC_GEMM_SPLIT3 ? 3 : (precision == SC_GEMM_SPLIT2 ? 2 : 1);
-  CUtensorMap ah, al, bh, bl;
-  if (int r = make_plane_map(&ah, a_hi, M, K, lda, BM)) return r;
-  if (int r = make_plane_map(&bh, b_hi, N, K, ldb, BN)) return r;
-  al = ah;
-  bl = bh;
-  if (prec >= 2) {
-    SC_REQUIRE(a_lo, "wgmma GEMM: the lo plane of A is missing");
-    if (int r = make_plane_map(&al, a_lo, M, K, lda, BM)) return r;
-  }
-  if (prec == 3) {
-    SC_REQUIRE(b_lo, "wgmma GEMM: the lo plane of B is missing");
-    if (int r = make_plane_map(&bl, b_lo, N, K, ldb, BN)) return r;
-  }
   const int m = (int)M, n = (int)N, k = (int)K;
   // C = Y Y^T is symmetric when both operands are the same matrix: compute the upper tiles only
   const bool sym = symmetric && a_hi == b_hi && a_lo == b_lo && M == N && lda == ldb;
   SC_REQUIRE(!(sym && mirror), "wgmma GEMM: a mirrored copy only makes sense for an off-diagonal block");
-#define SC_TC_LAUNCH(PR, EP, SY)                                                                 \
-  return launch<PR, EP, SY>(ctx, ah, al, bh, bl, m, n, k, C, ldc, rowmax_offdiag, diag_shift,    \
-                            stat_rowmax, stat_rowsum, mirror, ldm, st)
-#define SC_TC_PREC(PR)                                                                        \
-  do {                                                                                        \
-    if (epi == TC_EPI_AFFINITY) { if (sym) SC_TC_LAUNCH(PR, TC_EPI_AFFINITY, true);           \
-                                  SC_TC_LAUNCH(PR, TC_EPI_AFFINITY, false); }                 \
-    if (sym) SC_TC_LAUNCH(PR, TC_EPI_PLAIN, true);                                            \
-    SC_TC_LAUNCH(PR, TC_EPI_PLAIN, false);                                                    \
+#define SC_TC_LAUNCH(PR, EP, BN_)                                                                \
+  do {                                                                                           \
+    if (sym)                                                                                     \
+      return launch<PR, EP, true, BN_>(ctx, a_hi, a_lo, lda, b_hi, b_lo, ldb, m, n, k, C, ldc,   \
+                                       rowmax_offdiag, diag_shift, stat_rowmax, stat_rowsum,     \
+                                       mirror, ldm, st);                                         \
+    return launch<PR, EP, false, BN_>(ctx, a_hi, a_lo, lda, b_hi, b_lo, ldb, m, n, k, C, ldc,    \
+                                      rowmax_offdiag, diag_shift, stat_rowmax, stat_rowsum,      \
+                                      mirror, ldm, st);                                          \
   } while (0)
-  if (prec == 3) SC_TC_PREC(3);
-  if (prec == 2) SC_TC_PREC(2);
-  SC_TC_PREC(1);
-#undef SC_TC_PREC
+  // tile width per product: see the header
+  if (epi == TC_EPI_AFFINITY) {
+    if (precision == SC_GEMM_SPLIT3) SC_TC_LAUNCH(3, TC_EPI_AFFINITY, 128);
+    if (precision == SC_GEMM_SPLIT2) SC_TC_LAUNCH(2, TC_EPI_AFFINITY, 128);
+    SC_TC_LAUNCH(1, TC_EPI_AFFINITY, 128);
+  }
+  if (precision == SC_GEMM_SPLIT3) SC_TC_LAUNCH(3, TC_EPI_PLAIN, 128);
+  if (precision == SC_GEMM_SPLIT2) SC_TC_LAUNCH(2, TC_EPI_PLAIN, 192);
+  SC_TC_LAUNCH(1, TC_EPI_PLAIN, 192);
 #undef SC_TC_LAUNCH
 }
 
