@@ -329,6 +329,34 @@ int sc_kmeans(sc_context* ctx, const double* e, int64_t n, int64_t k_dim, int64_
               int64_t max_iter, double tol, int64_t* labels_host, int64_t* iters_host,
               void* stream);
 
+/* ---- AgglomerativeClustering(metric="cosine", linkage="complete") ------------------------
+ * The max_spectral_size pre-clustering (spectral_clusterer.py:211-220) and the pre-clusterer of
+ * MultiStageClusterer (multi_stage_clusterer.py:64,84).  scikit-learn runs it as
+ * scipy.spatial.distance.pdist(x, "cosine") followed by scipy.cluster.hierarchy.linkage(...,
+ * "complete"), i.e. scipy's _hierarchy.nn_chain; these two entries restate those two steps.  The
+ * sort of the merges, the relabelling and the tree cut are host logic
+ * (spectralcluster_b200/agglomerative.py). */
+
+/* dist[i,j] = 1 - clamp(x_i.x_j / (|x_i| |x_j|), -1, 1) for all i, j < n: scipy's pdist(x, "cosine")
+ * as a full symmetric fp64 matrix [n, ldd] (ldd >= n), 0 on the diagonal.  x is [n,d] fp32 (x_is_f64=0) or fp64 (=1), converted to double; norms are
+ * sqrt(sum x^2).  Products on the fp64 tensor cores; only the upper tiles are computed and each
+ * value is stored at (i,j) and (j,i), so dist is bitwise symmetric.  *nonfinite_flag (a device
+ * int) is set to 1 if any entry is not finite (a zero row, for instance) and to 0 otherwise. */
+int sc_cosine_distances_f64(sc_context* ctx, const void* x, int x_is_f64, int64_t n, int64_t d,
+                            int64_t ldx, double* dist, int64_t ldd, int* nonfinite_flag,
+                            void* stream);
+
+/* Complete-linkage NN-chain (scipy/cluster/_hierarchy.pyx nn_chain) over the finite symmetric
+ * fp64 matrix dist [n, ldd] (2 <= n < 2^31), all n - 1 merges in one cooperative launch.  The
+ * chain starts at the lowest active index; the nearest neighbour of the chain top x is the argmin
+ * of dist[x, i] over active i != x, where the previous chain element wins ties and otherwise the
+ * lowest index does.  Mutual neighbours x < y merge into y (x is retired) and dist[y,:] =
+ * dist[:,y] = max(dist[x,:], dist[y,:]).  Merge k, in chain order (unsorted, unrelabelled), goes to
+ * the HOST arrays merge_xy[2k], merge_xy[2k+1] (x < y), merge_dist[k] and merge_size[k] (points
+ * in the merged cluster).  dist is overwritten.  SYNCHRONOUS. */
+int sc_complete_linkage(sc_context* ctx, double* dist, int64_t n, int64_t ldd, int64_t* merge_xy,
+                        double* merge_dist, int64_t* merge_size, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

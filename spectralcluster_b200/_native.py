@@ -93,6 +93,9 @@ PROTOTYPES = {
     "sc_row_renorm": [c_ptr, c_ptr, c_i64, c_i64, c_ptr],
     "sc_kmeans": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64, c_int, c_i64, c_dbl,
                   c_ptr, c_ptr, c_ptr],
+    "sc_cosine_distances_f64": [c_ptr, c_ptr, c_int, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr,
+                                c_ptr],
+    "sc_complete_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
 }
 
 # enum values of include/spectralcluster_b200.h

@@ -148,4 +148,12 @@ __device__ __forceinline__ float ld_stream1(const float* p) {
   return r;
 }
 
+// C[8x8] += A[8x4] B[4x8] on the fp64 tensor cores (mma.sync m8n8k4; SASS DMMA).  Lane l holds
+// A[l/4][l%4], B[l%4][l/4] (B column-major) and C[l/4][2(l%4)], C[l/4][2(l%4)+1] in (c0, c1).
+__device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
+               : "+d"(c0), "+d"(c1)
+               : "d"(a), "d"(b));
+}
+
 }  // namespace sc

@@ -239,12 +239,6 @@ k_panel_w(int64_t n, int64_t j, int k, const double* __restrict__ tau, const dou
 constexpr int UPD_T = 64;
 constexpr int UPD_PITCH = 2 * NB + 4;     // doubles; == 4 mod 16: conflict-free 64-bit fragment loads
 
-__device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
-}
-
 __global__ void __launch_bounds__(256)
 k_trailing_update(double* __restrict__ a, int64_t n, int64_t lo, int kc,
                   const double* __restrict__ vv, const double* __restrict__ ww) {

@@ -138,6 +138,8 @@ class Engine:
       "sc_kmeans": "custom_distance_kmeans.run_kmeans", "sc_row_renorm": "spectral_clusterer.row_wise_renorm",
       "sc_affinity_stats": "fallback_clusterer.check_single_cluster",
       "sc_constraint_combine": "constraint.adjust_affinity", "sc_scale_shift": "constraint.adjust_affinity",
+      "sc_cosine_distances_f64": "AgglomerativeClustering(cosine, complete)",
+      "sc_complete_linkage": "AgglomerativeClustering(cosine, complete)",
   }
   nvtx = os.environ.get("SCB_NVTX") == "1"
 
@@ -388,6 +390,28 @@ class Engine:
               int(max_iter), float(tol), labels.ctypes.data_as(ctypes.c_void_p),
               iters.ctypes.data_as(ctypes.c_void_p), self.stream, exc=ValueError)
     return labels, int(iters[0])
+
+  def cosine_distances(self, x_dev):
+    """scipy pdist(x, "cosine") of a device [n, d] fp32/fp64 tensor as a full symmetric fp64
+    [n, ld] device matrix, and a device int32 flag that is 1 iff an entry is not finite."""
+    t = torch()
+    n, d = int(x_dev.shape[0]), int(x_dev.shape[1])
+    dist = self.matrix(n, t.float64)
+    flag = t.empty((1,), dtype=t.int32, device=self.device)
+    self.call("sc_cosine_distances_f64", _ptr(x_dev), 1 if x_dev.dtype == t.float64 else 0, n, d,
+              x_dev.stride(0), _ptr(dist), dist.stride(0), _ptr(flag), self.stream)
+    return dist, flag
+
+  def complete_linkage(self, dist, n: int):
+    """Complete-linkage NN-chain over the device distance matrix (overwritten) -> host
+    (xy int64 [n-1, 2], distance fp64 [n-1], size int64 [n-1]), in chain order."""
+    xy = np.empty((n - 1, 2), dtype=np.int64)
+    md = np.empty(n - 1, dtype=np.float64)
+    ms = np.empty(n - 1, dtype=np.int64)
+    self.call("sc_complete_linkage", _ptr(dist), n, dist.stride(0),
+              xy.ctypes.data_as(ctypes.c_void_p), md.ctypes.data_as(ctypes.c_void_p),
+              ms.ctypes.data_as(ctypes.c_void_p), self.stream)
+    return xy, md, ms
 
 
 class Refined:

@@ -5,8 +5,9 @@ MultiStageClusterer :67-180; Wang et al., arXiv:2210.13690).
 Per incoming embedding: fallback clusterer for short inputs (L), the spectral clusterer up to U1
 embeddings, beyond that an agglomerative pre-clusterer compresses the cache to U1 centroids which
 the spectral clusterer (device path) labels; the cache itself is replaced by its centroids every
-time it reaches U2.  Host logic and scikit-learn AHC around `SpectralClusterer.predict`, exactly as
-in the reference -- the matrices it hands to the device never exceed U1 x U1.
+time it reaches U2.  Host logic around `SpectralClusterer.predict` exactly as in the reference; the
+complete-linkage cosine pre-clusterer runs on the device with scikit-learn's labels
+(agglomerative.py).
 """
 
 from __future__ import annotations
@@ -15,6 +16,7 @@ import enum
 
 import numpy as np
 
+from . import agglomerative
 from . import fallback_clusterer
 from . import utils
 
@@ -49,7 +51,6 @@ class MultiStageClusterer:
 
   def __init__(self, main_clusterer, fallback_threshold: float = 0.5, L: int = 50, U1: int = 100,
                U2: int = 600, deflicker: Deflicker = Deflicker.NoDeflicker):
-    from sklearn.cluster import AgglomerativeClustering
     self.deflicker = deflicker
     self.main = main_clusterer
     if self.main.max_spectral_size:
@@ -61,7 +62,7 @@ class MultiStageClusterer:
     options.single_cluster_condition = fallback_clusterer.SingleClusterCondition.FallbackClusterer
     options.fallback_clusterer_type = fallback_clusterer.FallbackClustererType.Agglomerative
     self.U1, self.U2 = U1, U2
-    self.pre = AgglomerativeClustering(n_clusters=U1, metric="cosine", linkage="complete")
+    self.pre = agglomerative.CosineCompleteLinkage(n_clusters=U1)
     self.cache = None                    # embeddings, or centroids after a compression
     self.num_embeddings = 0
     self.compression_labels = None       # original embedding -> row of the cache

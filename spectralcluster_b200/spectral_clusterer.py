@@ -5,9 +5,10 @@ _compute_eigenvectors_ncluster :108-168, predict :201-314) whose arithmetic runs
 predict(): one H2D copy of the [N, d] embeddings, every N x N intermediate stays in HBM
 (affinity GEMM -> fused refinement -> Diffuse GEMM -> row statistics -> symmetric eigensolve ->
 k-means), one D2H copy of N labels.  The callers around the path follow the reference: the
-fallback clusterer for tiny inputs and the max_spectral_size AHC pre-clustering are host code
-(scikit-learn, as in the reference), the single-cluster checks are device reductions over the
-resident affinity.
+fallback clusterer for tiny inputs is host code (scikit-learn, as in the reference); the
+max_spectral_size AHC pre-clustering runs on the device (agglomerative.py: fp64 cosine distances and
+the complete-linkage NN-chain, scikit-learn's labels integer for integer); the single-cluster checks
+are device reductions over the resident affinity.
 """
 
 from __future__ import annotations
@@ -17,6 +18,7 @@ import typing
 import numpy as np
 
 from . import _native as nat
+from . import agglomerative
 from . import autotune as autotune_lib
 from . import constraint as constraint_lib
 from . import custom_distance_kmeans
@@ -210,12 +212,11 @@ class SpectralClusterer:
 
   def _reduce_size_and_predict(self, embeddings: np.ndarray) -> np.ndarray:
     """spectral_clusterer.py:170-199: complete-linkage cosine AHC down to `max_spectral_size`
-    clusters (scikit-learn, host -- the reference's own lossy answer to large N; the device path
-    does not need it, BASELINE configs[3] shards the exact problem instead), spectral clustering
-    of the cluster centroids on the device, labels chained back."""
-    from sklearn.cluster import AgglomerativeClustering
-    pre = AgglomerativeClustering(n_clusters=self.max_spectral_size, metric="cosine",
-                                  linkage="complete").fit_predict(embeddings)
+    clusters (the reference's own lossy answer to large N, on the device with scikit-learn's labels
+    -- see agglomerative.py; BASELINE configs[3] shards the exact problem instead), spectral
+    clustering of the cluster centroids on the device, labels chained back."""
+    pre = agglomerative.CosineCompleteLinkage(
+        n_clusters=self.max_spectral_size).fit_predict(embeddings)
     centroids = utils.get_cluster_centroids(embeddings, pre)
     return utils.chain_labels(pre, self.predict(centroids))
 
