@@ -659,6 +659,8 @@ __global__ void k_noblur(const BlurArgs g) {
 // Element-wise threshold + symmetrize on the stored upper half of B (EPI_UPPER), 64 x 64 tiles
 // with TI <= TJ: y = rule(b, m_i, m_j) is symmetric in (i, j), so the tile is written directly and,
 // for TI < TJ, once more transposed (through shared memory, 128-byte row segments of the planes).
+// A diagonal tile (TI == TJ) evaluates its lower half from the stored upper elements, so every pair
+// (i, j), (j, i) comes from the one b[min(i, j), max(i, j)] and Y is bitwise symmetric.
 constexpr int UT = 64;
 
 struct UpperArgs {
@@ -747,6 +749,13 @@ k_thrsym_upper(const UpperArgs g) {
       } else {
 #pragma unroll
         for (int t = 0; t < 4; ++t) bv[t] = (j + t < g.n) ? g.b[i * g.ldb + j + t] : 0.0f;
+      }
+      if (diag_tile) {
+        // below the diagonal, the mirror of the upper element: the computed blur is not bitwise
+        // symmetric, and Y(i, j) must equal Y(j, i) = rule(b[j, i], m_j, m_i) exactly
+#pragma unroll
+        for (int t = 0; t < 4; ++t)
+          if (j + t < i) bv[t] = g.b[(j + t) * g.ldb + i];
       }
       const float cut_i = g.m[i] * g.p;
 #pragma unroll
