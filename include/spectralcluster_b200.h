@@ -357,6 +357,40 @@ int sc_cosine_distances_f64(sc_context* ctx, const void* x, int x_is_f64, int64_
 int sc_complete_linkage(sc_context* ctx, double* dist, int64_t n, int64_t ldd, int64_t* merge_xy,
                         double* merge_dist, int64_t* merge_size, void* stream);
 
+/* ---- fallback_clusterer.check_single_cluster, AffinityGmmBic (fallback_clusterer.py:158-178) --
+ * scikit-learn's GaussianMixture(1) and (2) fitted to affinity[np.triu_indices(n, offset)], as
+ * one streaming reduction per step; the KMeans / EM / BIC control flow is host logic
+ * (spectralcluster_b200/gmm_bic.py).  A pass reads the band j >= max(0, i + offset), j < n of the
+ * fp32 matrix a [n, lda] and nothing else, promotes each sample x to fp64 and sums in fp64 in a
+ * fixed order (repeated calls agree bit for bit).  params_host[16] and out_host[8] are HOST
+ * arrays; work is a DEVICE fp64 buffer of 8 n + 8 elements, whose first n elements a KPP pass
+ * leaves for the LOOKUP that follows it.  "Centred" means x - p[0].  SYNCHRONOUS.
+ *   MOMENTS  p: shift s.  out: count, sum (x-s), sum (x-s)^2, min x, max x, #non-finite x.
+ *   KPP      p: mean, c0, ca, cb, trials (0 or 2), centres centred.  With d(c) = sklearn's
+ *            max(-2 x c + c^2 + x^2, 0) on centred x: out sum d(c0), sum min(d(c0), d(ca)),
+ *            sum min(d(c0), d(cb)) (the last two only if trials == 2).
+ *   LOOKUP   p: mean, c0, kind, v0, v1.  kind 0: v are flat band indices.  kind 1: v are targets
+ *            t and the index is searchsorted(cumsum(d(c0)), t) (count of prefixes below t),
+ *            summed row sums first, then within one row; clipped to m - 1.
+ *            out: index(v0), index(v1), x at each index.
+ *   LLOYD    p: mean, c0, c1, o0, o1, has_old (centred).  label(c) = argmin_k c_k^2 - 2 x c_k
+ *            (first minimum).  out: #label 1, sum x over label 0, over label 1 (centred x),
+ *            #label(c) != label(o) (0 without has_old).
+ *   LABELS   p: mean, c0, c1, s0, s1.  out: #label 1, sum x over label 0, over 1 (x not
+ *            centred), sum (x - s0)^2 over label 0, sum (x - s1)^2 over label 1.
+ *   EM       p: K (1 or 2), then per component: log w, mu pc, pc, log pc, shift.  With
+ *            w_k(x) = -0.5 (log 2 pi + (x pc - mu pc)^2) + log pc + log w and
+ *            lse = logsumexp_k w_k, r_k = exp(w_k - lse): out sum lse, then per component
+ *            sum r_k, sum r_k x, sum r_k (x - shift_k)^2.
+ *   SCORE    p as EM.  out: sum lse. */
+enum sc_gmm_mode {
+  SC_GMM_MOMENTS = 0, SC_GMM_KPP = 1, SC_GMM_LOOKUP = 2, SC_GMM_LLOYD = 3, SC_GMM_LABELS = 4,
+  SC_GMM_EM = 5, SC_GMM_SCORE = 6
+};
+int sc_gmm_band_pass(sc_context* ctx, const float* a, int64_t n, int64_t lda, int64_t offset,
+                     int mode, const double* params_host, double* work, double* out_host,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -148,6 +148,16 @@ __device__ __forceinline__ float ld_stream1(const float* p) {
   return r;
 }
 
+// squared distance in sklearn's expanded form (_euclidean_distances): |c|^2 - 2 x.c + |x|^2, >= 0
+__device__ __forceinline__ double sqdist_expanded(const double* __restrict__ x, int64_t i,
+                                                  int64_t kd, const double* __restrict__ c,
+                                                  double csq, double xsq_i) {
+  double dot = 0.0;
+  for (int64_t f = 0; f < kd; ++f) dot = fma(x[i * kd + f], c[f], dot);
+  const double v = csq - 2.0 * dot + xsq_i;
+  return v > 0.0 ? v : 0.0;
+}
+
 // C[8x8] += A[8x4] B[4x8] on the fp64 tensor cores (mma.sync m8n8k4; SASS DMMA).  Lane l holds
 // A[l/4][l%4], B[l%4][l/4] (B column-major) and C[l/4][2(l%4)], C[l/4][2(l%4)+1] in (c0, c1).
 __device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, double b) {

@@ -56,16 +56,6 @@ __global__ void k_center(const double* __restrict__ e, int64_t n, int64_t kd,
 }
 
 // ---- k-means++ ---------------------------------------------------------------------------
-// squared distance in sklearn's expanded form (_euclidean_distances): |c|^2 - 2 x.c + |x|^2, >= 0
-__device__ __forceinline__ double sqdist_expanded(const double* __restrict__ x, int64_t i,
-                                                  int64_t kd, const double* __restrict__ c,
-                                                  double csq, double xsq_i) {
-  double dot = 0.0;
-  for (int64_t f = 0; f < kd; ++f) dot = fma(x[i * kd + f], c[f], dot);
-  const double v = csq - 2.0 * dot + xsq_i;
-  return v > 0.0 ? v : 0.0;
-}
-
 // closest[i] = d2(x_i, x_first); partial sums per block -> part[block]
 __global__ void k_kpp_first(const double* __restrict__ x, const double* __restrict__ xsq,
                             int64_t n, int64_t kd, int64_t first, double* __restrict__ closest,

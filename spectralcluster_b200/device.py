@@ -137,6 +137,7 @@ class Engine:
       "sc_eigh_extremal_sharded": "utils.compute_sorted_eigenvectors",
       "sc_kmeans": "custom_distance_kmeans.run_kmeans", "sc_row_renorm": "spectral_clusterer.row_wise_renorm",
       "sc_affinity_stats": "fallback_clusterer.check_single_cluster",
+      "sc_gmm_band_pass": "fallback_clusterer.check_single_cluster",
       "sc_constraint_combine": "constraint.adjust_affinity", "sc_scale_shift": "constraint.adjust_affinity",
       "sc_cosine_distances_f64": "AgglomerativeClustering(cosine, complete)",
       "sc_complete_linkage": "AgglomerativeClustering(cosine, complete)",

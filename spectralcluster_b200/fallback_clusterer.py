@@ -5,8 +5,10 @@
 What runs where:
   * AllAffinity / NeighborAffinity / AffinityStd are reductions over the N x N affinity: one
     streaming pass on the device (`sc_affinity_stats`), four doubles come back;
-  * AffinityGmmBic fits scikit-learn GMMs to the N^2/2 upper-triangular affinities: host, on a
-    copy of the device affinity (SURVEY.md 8(f)-4: "keep on host");
+  * AffinityGmmBic fits 1- and 2-component GMMs to the N^2/2 upper-band affinities: on the
+    device for a device-resident affinity, one streaming pass per KMeans / EM step
+    (`gmm_bic`, `sc_gmm_band_pass`), with scikit-learn's arithmetic and random draws; a host
+    ndarray still goes to scikit-learn;
   * FallbackClusterer (scikit-learn average-linkage AHC, or the sequential naive clusterer) only
     ever sees inputs below `spectral_min_embeddings` or acts as a probe: host.
 """
@@ -89,10 +91,13 @@ def affinity_statistics(affinity) -> typing.Dict[str, float]:
 
 
 def check_single_cluster(fallback_options: FallbackOptions,
-                         embeddings: typing.Optional[np.ndarray], affinity) -> bool:
+                         embeddings: typing.Optional[np.ndarray], affinity,
+                         details: typing.Optional[dict] = None) -> bool:
   """True when the data form a single cluster (only consulted when min_clusters == 1).
 
-  `affinity` is a host ndarray (reference signature) or the DeviceAffinity predict() holds."""
+  `affinity` is a host ndarray (reference signature) or the DeviceAffinity predict() holds.
+  For AffinityGmmBic on a device affinity, `details` (if given) receives the two BICs, both
+  GMMs' EM iteration counts and the number of passes over the affinity."""
   cond = fallback_options.single_cluster_condition
   thr = fallback_options.single_cluster_affinity_threshold
   if cond == SingleClusterCondition.AllAffinity:
@@ -102,15 +107,19 @@ def check_single_cluster(fallback_options: FallbackOptions,
   if cond == SingleClusterCondition.AffinityStd:
     return affinity_statistics(affinity)["std"] < thr
   if cond == SingleClusterCondition.AffinityGmmBic:
-    from sklearn.mixture import GaussianMixture
-    if not isinstance(affinity, np.ndarray):
-      from . import device as dev
-      affinity = dev.Engine.get().download_matrix(affinity.matrix, affinity.n)
-    n = affinity.shape[0]
+    n = affinity.shape[0] if isinstance(affinity, np.ndarray) else affinity.n
     offset = fallback_options.single_cluster_affinity_diagonal_offset
     if offset >= n - 1:
       raise ValueError("single_cluster_affinity_diagonal_offset must be significantly "
                        "smaller than affinity matrix dimension")
+    if not isinstance(affinity, np.ndarray):
+      from . import device as dev
+      from . import gmm_bic
+      res = gmm_bic.gmm_bic(gmm_bic.DeviceOps(dev.Engine.get(), affinity.matrix, n, offset))
+      if details is not None:
+        details.update(bic=res.bic, n_iter=res.n_iter, passes=res.passes)
+      return res.single
+    from sklearn.mixture import GaussianMixture
     values = affinity[np.triu_indices(n, offset)][:, None]
     bic = [GaussianMixture(n_components=c).fit(values).bic(values) for c in (1, 2)]
     return bool(bic[0] < bic[1])

@@ -266,9 +266,13 @@ class SpectralClusterer:
       affinity = DeviceAffinity(eng.upload_matrix(host), num_embeddings, None,
                                 bool(np.allclose(host, host.T, rtol=1e-6, atol=1e-9)))
 
+    single_details = {}
     if self.min_clusters == 1:
       # single-vs-multi cluster decision on the resident affinity (spectral_clusterer.py:253-256)
-      if fallback_clusterer.check_single_cluster(self.fallback_options, embeddings, affinity):
+      if fallback_clusterer.check_single_cluster(self.fallback_options, embeddings, affinity,
+                                                 single_details):
+        if single_details:
+          self.last_details = dict(single_cluster=single_details)
         return np.array([0] * num_embeddings)
 
     if (self.constraint_options and self.constraint_options.apply_before_refinement and
@@ -292,12 +296,17 @@ class SpectralClusterer:
         raise ValueError("Unsupported value of AutoTuneProxy")
 
       if self.autotune_group is not None:
-        return self._predict_parallel_autotune(eng, affinity, p_percentile_to_ratio)
+        labels = self._predict_parallel_autotune(eng, affinity, p_percentile_to_ratio)
+        if single_details:
+          self.last_details["single_cluster"] = single_details
+        return labels
       eigenvectors, n_clusters, best_p = self.autotune.tune(p_percentile_to_ratio)
       self.last_details["best_p_percentile"] = best_p
     else:
       eigenvectors, n_clusters, _ = self._compute_eigenvectors_ncluster(affinity, constraint_matrix)
     del affinity
+    if single_details:
+      self.last_details["single_cluster"] = single_details
 
     return self._cluster_embeddings(eng, eigenvectors, n_clusters)
 
