@@ -14,12 +14,14 @@
 // blurred -- ONCE.  Pass 1 reads half of A, stores that half of B and folds both the row maxima
 // and the column maxima of every tile into m (m_i = max_j B_ij needs the lower half only through
 // B_ji).  Pass 2 is element-wise on the stored half of B and writes Y(i,j) and Y(j,i) (transposed
-// through shared memory).  HBM traffic 2 + 2 + 2 + 4 = 10 B per element of the matrix (the
-// contract figure is 12) and half the filter arithmetic of the two-pass form; both kernels were
+// through shared memory).  HBM traffic 2 + 2 + 2 + 2 = 8 B per element of the matrix when only the
+// hi plane of Y is written (a single-MMA Diffuse follows; 10 B with the lo plane, the contract
+// figure is 12) and half the filter arithmetic of the two-pass form; both kernels were
 // issue-bound, not bandwidth-bound.
 //
-// Two kernels: k_blur_tile<R> (compile-time radius, register sliding windows; R=4 is sigma=1,
-// the configuration every BASELINE config uses) and k_blur_generic (run-time radius <= 64).
+// Kernels: k_blur_band<4, EPI> (compile-time radius 4 = sigma ~ 1, the configuration every
+// BASELINE config uses: register sliding windows, cp.async pipeline), k_blur_generic<EPI>
+// (run-time radius <= 64), k_noblur<EPI> (radius 0 and sigma <= 1e-15) and k_thrsym_upper.
 #include "common.cuh"
 
 #include <cstdlib>
@@ -27,6 +29,18 @@
 namespace sc {
 
 constexpr int kMaxRadius = 64;
+
+// The threshold/symmetrize rule and the Y outputs, shared by every kernel that writes Y.
+struct RuleArgs {
+  const float* m;          // row maxima of the blurred matrix
+  float p, mult;
+  int binarize, preserve_diag, sym_type;
+  float* y;                // fp32 Y (optional)
+  int64_t ldy;
+  __half* hi;              // split fp16 planes of Y (optional; lo optional even with hi)
+  __half* lo;
+  int64_t ldh;
+};
 
 struct BlurArgs {
   const float* a;          // rows [in_row_base, ...) of the global n x n matrix
@@ -37,19 +51,12 @@ struct BlurArgs {
   int64_t row_begin, row_end, in_row_base, out_row_base;
   const float* diag;       // optional replacement of a[i][i]
   int radius;
-  float* out;              // EPI_STORE
+  float* out;              // EPI_STORE / EPI_UPPER
   int64_t ldo;
-  float* rowmax_out;       // EPI_STORE (optional) / EPI_STATS
-  // threshold + symmetrize epilogue
-  const float* m;          // row maxima of the blurred matrix
-  float p, mult;
-  int binarize, preserve_diag, sym_type, stats_zero_diag;
+  float* rowmax_out;       // EPI_STORE (optional) / EPI_STATS / EPI_UPPER
+  int stats_zero_diag;
   int tiles_per_cta;       // column tiles swept by one CTA of k_blur_band (cp.async pipeline)
-  float* y;
-  int64_t ldy;
-  __half* hi;
-  __half* lo;
-  int64_t ldh;
+  RuleArgs r;              // EPI_THRSYM
 };
 
 struct BlurWeights {
@@ -66,37 +73,99 @@ __device__ __forceinline__ int64_t reflect_index(int64_t i, int64_t n) {
   return (i < n) ? i : (period - 1 - i);
 }
 
-__device__ __forceinline__ float threshold_rule(float b, float m, float p, float mult,
-                                                int binarize) {
-  return (b < m * p) ? b * mult : (binarize ? 1.0f : b);
+// y = sym(thr(b, m_i), thr(b, m_j)), thr(b, m) = b < m p ? b mult : (binarize ? 1 : b)
+// (SURVEY.md A.3).  Every caller forms the cuts as the fp32 products m_i * p and m_j * p.
+// `diag` marks the element (i, i), which preserve_diagonal sets to 1 (refinement.py:208-209).
+__device__ __forceinline__ float thrsym_rule(const RuleArgs& r, float b, float cut_i, float cut_j,
+                                             bool diag) {
+  const float keep = r.binarize ? 1.0f : b;
+  const float small = b * r.mult;
+  const float t1 = (b < cut_i) ? small : keep;
+  const float t2 = (b < cut_j) ? small : keep;
+  const float y = (r.sym_type == SC_SYMMETRIZE_MAX) ? fmaxf(t1, t2) : 0.5f * (t1 + t2);
+  return (diag && r.preserve_diag) ? 1.0f : y;
+}
+
+// dst[0 .. N) <- w[] (N 32-bit words, dst aligned to the store): 128-bit stores, or one 64-bit store
+// for N = 2.  Written as PTX because the compiler, given the same stores as C++, merged the
+// identical epilogues of the edge and interior tiles of k_blur_band and split the first 128-bit
+// store of every run into four 32-bit ones, which made the kernels 1.5x slower.
+template <int N>
+__device__ __forceinline__ void store_words(void* dst, const uint32_t (&w)[N]) {
+  static_assert(N == 2 || N % 4 == 0, "64-bit or 128-bit stores");
+  if constexpr (N == 2) {
+    asm volatile("st.global.v2.b32 [%0], {%1, %2};" ::"l"(dst), "r"(w[0]), "r"(w[1]) : "memory");
+  } else {
+#pragma unroll
+    for (int q = 0; q < N / 4; ++q)
+      asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};"
+                   ::"l"(static_cast<uint32_t*>(dst) + 4 * q), "r"(w[4 * q]), "r"(w[4 * q + 1]),
+                     "r"(w[4 * q + 2]), "r"(w[4 * q + 3])
+                   : "memory");
+  }
+}
+
+template <int N>
+__device__ __forceinline__ void store_floats(float* dst, const float (&v)[N]) {
+  uint32_t w[N];
+#pragma unroll
+  for (int t = 0; t < N; ++t) w[t] = __float_as_uint(v[t]);
+  store_words<N>(dst, w);
+}
+
+// Y(io, j0 .. j0 + W - 1) <- y[]: fp32 and/or the split planes hi = fp16(y), lo = fp16(y - hi).
+// A complete run (`full`) goes out as vector stores (W = 16: two 128-bit stores per plane, W = 4:
+// one 64-bit store); otherwise element by element, stopping at column n.
+template <int W>
+__device__ __forceinline__ void store_y(const RuleArgs& r, int64_t io, int64_t j0,
+                                        const float (&y)[W], bool full, int64_t n) {
+  static_assert(W == 1 || W == 4 || W == 16, "runs of 1, 4 or 16 values");
+  if constexpr (W > 1) {
+    if (full) {
+      if (r.y) store_floats<W>(r.y + io * r.ldy + j0, y);
+      if (r.hi) {
+        uint32_t hw[W / 2], lw[W / 2];
+#pragma unroll
+        for (int q = 0; q < W / 2; ++q) {
+          const __half2 h = __floats2half2_rn(y[2 * q], y[2 * q + 1]);
+          const float2 f = __half22float2(h);
+          const __half2 l = __floats2half2_rn(y[2 * q] - f.x, y[2 * q + 1] - f.y);
+          hw[q] = *reinterpret_cast<const uint32_t*>(&h);
+          lw[q] = *reinterpret_cast<const uint32_t*>(&l);
+        }
+        store_words<W / 2>(r.hi + io * r.ldh + j0, hw);
+        if (r.lo) store_words<W / 2>(r.lo + io * r.ldh + j0, lw);
+      }
+      return;
+    }
+  }
+#pragma unroll
+  for (int t = 0; t < W; ++t) {
+    if (!full && j0 + t >= n) continue;
+    if (r.y) r.y[io * r.ldy + j0 + t] = y[t];
+    if (r.hi) {
+      __half h, l;
+      split_half(y[t], h, l);
+      r.hi[io * r.ldh + j0 + t] = h;
+      if (r.lo) r.lo[io * r.ldh + j0 + t] = l;
+    }
+  }
 }
 
 // One output element (i, j) with blurred value b.  Returns the value that takes part in the
 // row maximum (EPI_STORE / EPI_STATS).
 template <int EPI>
 __device__ __forceinline__ float blur_epilogue(const BlurArgs& g, int64_t i, int64_t j, float b) {
+  static_assert(EPI != EPI_UPPER, "the symmetric pass runs on k_blur_band only");
   if (EPI == EPI_STORE) {
     g.out[(i - g.out_row_base) * g.ldo + j] = b;
     return b;
   } else if (EPI == EPI_STATS) {
     return (g.stats_zero_diag && i == j) ? 0.0f : b;   // RowWiseThreshold preserve_diagonal
   } else {
-    float yv;
-    if (g.preserve_diag && i == j) {
-      yv = 1.0f;                                        // refinement.py:208-209
-    } else {
-      const float t1 = threshold_rule(b, g.m[i], g.p, g.mult, g.binarize);
-      const float t2 = threshold_rule(b, g.m[j], g.p, g.mult, g.binarize);
-      yv = (g.sym_type == SC_SYMMETRIZE_MAX) ? fmaxf(t1, t2) : 0.5f * (t1 + t2);
-    }
-    if (g.y) g.y[(i - g.out_row_base) * g.ldy + j] = yv;
-    if (g.hi) {
-      __half h, l;
-      split_half(yv, h, l);
-      g.hi[(i - g.out_row_base) * g.ldh + j] = h;
-      g.lo[(i - g.out_row_base) * g.ldh + j] = l;
-    }
-    return yv;
+    const float y[1] = {thrsym_rule(g.r, b, g.r.m[i] * g.r.p, g.r.m[j] * g.r.p, i == j)};
+    store_y<1>(g.r, i - g.out_row_base, j, y, true, g.n);
+    return y[0];
   }
 }
 
@@ -158,46 +227,50 @@ k_blur_generic(const BlurArgs g, const BlurWeights bw) {
 // below the 4+8 B/element of HBM traffic the two passes of the fused chain are allowed.
 constexpr int TTH = 32, TTW = 128, TTHREADS = 288, VSTRIP = 16, HSTRIP = 16;
 
-template <int EPI>
+// The 16 blurred values b[] of row i, columns j0 .. j0 + 15.  Edge tiles (EDGE) check the columns
+// against n and the diagonal; the interior tiles of the fast path are complete and off-diagonal,
+// and all 32 lanes of each horizontal-pass warp reach the epilogue together.  `out_row` is row i of
+// B for the fast path's stores (FastCtx).
+template <int EPI, bool EDGE>
 __device__ __forceinline__ void epilogue16(const BlurArgs& g, int64_t i, int64_t j0,
-                                           const float (&b)[HSTRIP], float& rmax) {
-  const bool full = (j0 + HSTRIP <= g.n);
-  if (EPI == EPI_STATS) {
-    float v = rmax;
-#pragma unroll
-    for (int t = 0; t < HSTRIP; ++t) {
-      float x = b[t];
-      if (!full && j0 + t >= g.n) x = 0.0f;
-      if (g.stats_zero_diag && i == j0 + t) x = 0.0f;   // RowWiseThreshold preserve_diagonal
-      v = fmaxf(v, x);
-    }
-    rmax = v;
-    return;
-  }
+                                           const float (&b)[HSTRIP], float& rmax, float* out_row) {
+  const bool full = !EDGE || j0 + HSTRIP <= g.n;
   const int64_t io = i - g.out_row_base;
-  if (EPI == EPI_UPPER) {
-    // edge / diagonal tiles of the symmetric pass: store B, row maximum in the register, column
-    // maxima by one atomic per element (O(N) such tiles out of N^2/4096)
-    float* dst = g.out + io * g.ldo + j0;
-    float v = rmax;
+  if (EPI == EPI_STATS || EPI == EPI_UPPER) {
+    if (EPI == EPI_UPPER && !EDGE) store_floats<HSTRIP>(out_row + j0, b);
+    // EPI_UPPER also stores B and folds the column maxima of the tile into m: by one atomic per
+    // element on edge / diagonal tiles (O(N) such tiles out of N^2/4096)
 #pragma unroll
     for (int t = 0; t < HSTRIP; ++t) {
       if (!full && j0 + t >= g.n) continue;
-      dst[t] = b[t];
-      const float x = (g.stats_zero_diag && i == j0 + t) ? 0.0f : b[t];
-      v = fmaxf(v, x);
-      atomic_max_nonneg(g.rowmax_out + j0 + t, fmaxf(x, 0.0f));
+      // RowWiseThreshold preserve_diagonal
+      const float x = (EDGE && g.stats_zero_diag && i == j0 + t) ? 0.0f : b[t];
+      rmax = fmaxf(rmax, x);
+      if (EPI == EPI_UPPER && EDGE) {
+        g.out[io * g.ldo + j0 + t] = b[t];
+        atomic_max_nonneg(g.rowmax_out + j0 + t, fmaxf(x, 0.0f));
+      }
     }
-    rmax = v;
+    if (EPI == EPI_UPPER && !EDGE) {
+      // The lanes of this warp are the tile's 32 rows, each holding the same 16 columns.  The
+      // blurred values are non-negative, so their bit patterns order like signed integers and one
+      // REDUX.MAX per column reduces across the warp (16 instructions; the shuffle butterfly
+      // before it took ~95); lane t keeps column t and issues its atomic.
+      const int lane = threadIdx.x & 31;
+      float cm = 0.0f;
+#pragma unroll
+      for (int t = 0; t < HSTRIP; ++t) {
+        const int mx = __reduce_max_sync(0xffffffffu, __float_as_int(fmaxf(b[t], 0.0f)));
+        if (lane == t) cm = __int_as_float(mx);
+      }
+      if (lane < HSTRIP) atomic_max_nonneg(g.rowmax_out + j0 + lane, cm);
+    }
     return;
   }
   if (EPI == EPI_STORE) {
-    float* dst = g.out + io * g.ldo + j0;
+    float* dst = (EDGE ? g.out + io * g.ldo : out_row) + j0;
     if (full) {
-#pragma unroll
-      for (int q = 0; q < HSTRIP / 4; ++q)
-        *reinterpret_cast<float4*>(dst + 4 * q) =
-            make_float4(b[4 * q], b[4 * q + 1], b[4 * q + 2], b[4 * q + 3]);
+      store_floats<HSTRIP>(dst, b);
     } else {
 #pragma unroll
       for (int t = 0; t < HSTRIP; ++t)
@@ -212,72 +285,28 @@ __device__ __forceinline__ void epilogue16(const BlurArgs& g, int64_t i, int64_t
     }
     return;
   }
-  // EPI_THRSYM: y = sym(thr(b, m_i), thr(b, m_j))  (SURVEY.md A.3)
-  const float cut_i = g.m[i] * g.p;
+  // EPI_THRSYM
+  const RuleArgs& r = g.r;
+  const float cut_i = r.m[i] * r.p;
+  // column of the diagonal element within the run (-1: none): one range test instead of sixteen
+  // 64-bit compares, which the compiler hoists at a cost of ~30 registers
+  const int dcol = (EDGE && i >= j0 && i < j0 + HSTRIP) ? (int)(i - j0) : -1;
   float y[HSTRIP];
 #pragma unroll
   for (int q = 0; q < HSTRIP / 4; ++q) {
     float mj[4];
     if (full) {
-      const float4 v = *reinterpret_cast<const float4*>(g.m + j0 + 4 * q);   // warp-broadcast
+      const float4 v = *reinterpret_cast<const float4*>(r.m + j0 + 4 * q);   // warp-broadcast
       mj[0] = v.x; mj[1] = v.y; mj[2] = v.z; mj[3] = v.w;
     } else {
 #pragma unroll
-      for (int t = 0; t < 4; ++t) mj[t] = (j0 + 4 * q + t < g.n) ? g.m[j0 + 4 * q + t] : 0.0f;
+      for (int t = 0; t < 4; ++t) mj[t] = (j0 + 4 * q + t < g.n) ? r.m[j0 + 4 * q + t] : 0.0f;
     }
 #pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const float x = b[4 * q + t];
-      const float keep = g.binarize ? 1.0f : x;
-      const float small = x * g.mult;
-      const float t1 = (x < cut_i) ? small : keep;
-      const float t2 = (x < mj[t] * g.p) ? small : keep;
-      y[4 * q + t] = (g.sym_type == SC_SYMMETRIZE_MAX) ? fmaxf(t1, t2) : 0.5f * (t1 + t2);
-    }
+    for (int t = 0; t < 4; ++t)
+      y[4 * q + t] = thrsym_rule(r, b[4 * q + t], cut_i, mj[t] * r.p, dcol == 4 * q + t);
   }
-  if (g.preserve_diag) {
-#pragma unroll
-    for (int t = 0; t < HSTRIP; ++t)
-      if (i == j0 + t) y[t] = 1.0f;                       // refinement.py:208-209
-  }
-  if (full) {
-    if (g.y) {
-      float* dst = g.y + io * g.ldy + j0;
-#pragma unroll
-      for (int q = 0; q < HSTRIP / 4; ++q)
-        *reinterpret_cast<float4*>(dst + 4 * q) =
-            make_float4(y[4 * q], y[4 * q + 1], y[4 * q + 2], y[4 * q + 3]);
-    }
-    if (g.hi) {
-      uint32_t hw[HSTRIP / 2], lw[HSTRIP / 2];
-#pragma unroll
-      for (int q = 0; q < HSTRIP / 2; ++q) {
-        const __half2 h = __floats2half2_rn(y[2 * q], y[2 * q + 1]);
-        const float2 f = __half22float2(h);
-        const __half2 l = __floats2half2_rn(y[2 * q] - f.x, y[2 * q + 1] - f.y);
-        hw[q] = *reinterpret_cast<const uint32_t*>(&h);
-        lw[q] = *reinterpret_cast<const uint32_t*>(&l);
-      }
-      uint4* hd = reinterpret_cast<uint4*>(g.hi + io * g.ldh + j0);
-      uint4* ld = reinterpret_cast<uint4*>(g.lo + io * g.ldh + j0);
-      hd[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-      hd[1] = make_uint4(hw[4], hw[5], hw[6], hw[7]);
-      ld[0] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-      ld[1] = make_uint4(lw[4], lw[5], lw[6], lw[7]);
-    }
-  } else {
-#pragma unroll
-    for (int t = 0; t < HSTRIP; ++t) {
-      if (j0 + t >= g.n) continue;
-      if (g.y) g.y[io * g.ldy + j0 + t] = y[t];
-      if (g.hi) {
-        __half h, l;
-        split_half(y[t], h, l);
-        g.hi[io * g.ldh + j0 + t] = h;
-        g.lo[io * g.ldh + j0 + t] = l;
-      }
-    }
-  }
+  store_y<HSTRIP>(r, io, j0, y, full, g.n);
 }
 
 __device__ __forceinline__ void cp_async16(float* smem_dst, const float* gmem_src) {
@@ -307,6 +336,39 @@ __device__ __forceinline__ bool tile_is_vec(const BlurArgs& g, int64_t row0, int
          ((g.lda & 3) == 0) && ((reinterpret_cast<uintptr_t>(g.a) & 15) == 0);
 }
 
+// One thread's share of the two filter passes of a tile.
+struct PassOffsets {
+  int v_in, v_mid;             // vertical pass: first input / output element (-1: idle)
+  int h_mid, h_r, h_c0;        // horizontal pass: first `mid` element (-1: idle), row, strip column
+};
+
+template <int R>
+__device__ __forceinline__ PassOffsets pass_offsets(int tid) {
+  using G = TileGeom<R>;
+  PassOffsets o;
+  const int vc = tid % G::IW, vr0 = (tid / G::IW) * VSTRIP;
+  o.v_in = tid < G::IW * (TTH / VSTRIP) ? vr0 * G::IW + vc : -1;
+  o.v_mid = vr0 * G::MP + vc;
+  o.h_r = tid % TTH;
+  o.h_c0 = (tid / TTH) * HSTRIP;
+  o.h_mid = tid < TTH * (TTW / HSTRIP) ? o.h_r * G::MP + o.h_c0 : -1;
+  return o;
+}
+
+// ---- fast path: interior, off-diagonal, full tiles (all but O(N) of the N^2/4096 tiles).
+// Everything that does not change from tile to tile inside a band is hoisted into FastCtx; the
+// edge tiles recompute their pass offsets (cheaper than keeping them live across the edge path).
+template <int R>
+struct FastCtx {
+  static constexpr int FILL_ITERS = (TileGeom<R>::IH * (TileGeom<R>::IW / 4) + TTHREADS - 1) / TTHREADS;
+  int fill_smem[FILL_ITERS];   // float offset inside the tile buffer (-1: no copy this round)
+  int fill_gofs[FILL_ITERS];   // element offset from the tile's first source element
+  PassOffsets pass;
+  // row of B this thread stores (EPI_STORE / EPI_UPPER).  With the address formed per tile, the
+  // compiler shared it with the edge tiles' epilogue and the upper pass ran 1.15x slower.
+  float* out_row;
+};
+
 // Stage the halo'd input tile into `in`.  Interior tiles go through cp.async (16-byte copies
 // that complete in the background: the caller commits the group and waits before use); edge
 // tiles take the synchronous path with reflected indices.
@@ -330,85 +392,6 @@ __device__ __forceinline__ void tile_fill(const BlurArgs& g, int64_t row0, int64
   }
 }
 
-// Both separable passes + epilogue on a staged tile.  The caller has made `in` visible to the
-// whole block (cp.async.wait_group + __syncthreads) and guarantees nobody still reads `mid`.
-template <int R, int EPI>
-__device__ __forceinline__ void tile_compute(const BlurArgs& g, const float (&w)[2 * R + 1],
-                                             int64_t row0, int64_t col0, float* in, float* mid,
-                                             float& rmax) {
-  using G = TileGeom<R>;
-  const int tid = threadIdx.x;
-  if (g.diag && tile_is_vec<R>(g, row0, col0)) {
-    // fused CropDiagonal on the vector path: patch the diagonal elements inside the halo'd tile
-    const int64_t lo = (row0 > col0 ? row0 : col0) - R;
-    const int64_t hi = ((row0 + TTH < col0 + TTW) ? row0 + TTH : col0 + TTW) + R;
-    if (lo < hi) {                                     // block-uniform
-      for (int64_t d = lo + tid; d < hi; d += TTHREADS)
-        in[(d - (row0 - R)) * G::IW + (d - (col0 - R))] = g.diag[d];
-      __syncthreads();
-    }
-  }
-  if (tid < G::IW * (TTH / VSTRIP)) {
-    const int c = tid % G::IW, r0 = (tid / G::IW) * VSTRIP;
-    float win[VSTRIP + 2 * R];
-#pragma unroll
-    for (int k = 0; k < VSTRIP + 2 * R; ++k) win[k] = in[(r0 + k) * G::IW + c];
-#pragma unroll
-    for (int o = 0; o < VSTRIP; ++o) {
-      float acc = 0.0f;
-#pragma unroll
-      for (int k = 0; k <= 2 * R; ++k) acc = fmaf(w[k], win[o + k], acc);
-      mid[(r0 + o) * G::MP + c] = acc;
-    }
-  }
-  __syncthreads();
-  if (tid < TTH * (TTW / HSTRIP)) {
-    const int r = tid % TTH, c0 = (tid / TTH) * HSTRIP;
-    float win[HSTRIP + 2 * R];
-#pragma unroll
-    for (int k = 0; k < HSTRIP + 2 * R; ++k) win[k] = mid[r * G::MP + c0 + k];
-    float b[HSTRIP];
-#pragma unroll
-    for (int o = 0; o < HSTRIP; ++o) {
-      float acc = 0.0f;
-#pragma unroll
-      for (int k = 0; k <= 2 * R; ++k) acc = fmaf(w[k], win[o + k], acc);
-      b[o] = acc;
-    }
-    const int64_t i = row0 + r, j0 = col0 + c0;
-    if (i < g.row_end && j0 < g.n) epilogue16<EPI>(g, i, j0, b, rmax);
-  }
-}
-
-// ---- fast path: interior, off-diagonal, full tiles (all but O(N) of the N^2/4096 tiles).
-// Everything that does not change from tile to tile inside a band is hoisted into FastCtx, and
-// nothing is bounds-checked: the general tile_fill / tile_compute above remain the fallback for
-// edge tiles, tiles that touch the diagonal (CropDiagonal patch, preserve_diagonal) and ragged
-// row blocks.
-template <int R>
-struct FastCtx {
-  static constexpr int FILL_ITERS = (TileGeom<R>::IH * (TileGeom<R>::IW / 4) + TTHREADS - 1) / TTHREADS;
-  int fill_smem[FILL_ITERS];   // float offset inside the tile buffer (-1: no copy this round)
-  int fill_gofs[FILL_ITERS];   // element offset from the tile's first source element
-  int v_in, v_mid;             // vertical pass: first input / output element (-1: idle)
-  int h_mid, h_c0;             // horizontal pass: first `mid` element (-1: idle), strip column
-  float cut_i;                 // m[i] * p of this thread's output row (EPI_THRSYM)
-  float* y_row;                // output row bases of this thread's row
-  __half* hi_row;
-  __half* lo_row;
-  float* out_row;
-};
-
-template <int R>
-__device__ __forceinline__ bool tile_is_fast(const BlurArgs& g, int64_t row0, int64_t col0) {
-  if (!tile_is_vec<R>(g, row0, col0)) return false;
-  if (col0 + TTW > g.n || row0 + TTH > g.row_end) return false;
-  // tiles whose halo'd footprint meets the diagonal take the general path
-  const int64_t lo = (row0 > col0 ? row0 : col0) - R;
-  const int64_t hi = ((row0 + TTH < col0 + TTW) ? row0 + TTH : col0 + TTW) + R;
-  return lo >= hi;
-}
-
 template <int R>
 __device__ __forceinline__ void fast_fill(const FastCtx<R>& c, const float* src, float* in) {
 #pragma unroll
@@ -416,114 +399,67 @@ __device__ __forceinline__ void fast_fill(const FastCtx<R>& c, const float* src,
     if (c.fill_smem[k] >= 0) cp_async16(in + c.fill_smem[k], src + c.fill_gofs[k]);
 }
 
-template <int R, int EPI>
-__device__ __forceinline__ void fast_compute(const BlurArgs& g, const FastCtx<R>& c,
-                                             const float (&w)[2 * R + 1], int64_t col0,
-                                             const float* in, float* mid, float& rmax) {
+// Vertical pass of one thread: a register window slides down a column of `in` (pitch IW) and
+// VSTRIP outputs go down the same column of `mid` (pitch MP).
+template <int R>
+__device__ __forceinline__ void vertical_pass(const float (&w)[2 * R + 1], const float* in,
+                                              float* mid) {
   using G = TileGeom<R>;
-  if (c.v_in >= 0) {
-    float win[VSTRIP + 2 * R];
+  float win[VSTRIP + 2 * R];
 #pragma unroll
-    for (int k = 0; k < VSTRIP + 2 * R; ++k) win[k] = in[c.v_in + k * G::IW];
+  for (int k = 0; k < VSTRIP + 2 * R; ++k) win[k] = in[k * G::IW];
 #pragma unroll
-    for (int o = 0; o < VSTRIP; ++o) {
-      float acc = 0.0f;
+  for (int o = 0; o < VSTRIP; ++o) {
+    float acc = 0.0f;
 #pragma unroll
-      for (int k = 0; k <= 2 * R; ++k) acc = fmaf(w[k], win[o + k], acc);
-      mid[c.v_mid + o * G::MP] = acc;
+    for (int k = 0; k <= 2 * R; ++k) acc = fmaf(w[k], win[o + k], acc);
+    mid[o * G::MP] = acc;
+  }
+}
+
+// Horizontal pass of one thread: HSTRIP outputs along a row of `mid`.
+template <int R>
+__device__ __forceinline__ void horizontal_pass(const float (&w)[2 * R + 1], const float* mid,
+                                                float (&b)[HSTRIP]) {
+  float win[HSTRIP + 2 * R];
+#pragma unroll
+  for (int k = 0; k < HSTRIP + 2 * R; ++k) win[k] = mid[k];
+#pragma unroll
+  for (int o = 0; o < HSTRIP; ++o) {
+    float acc = 0.0f;
+#pragma unroll
+    for (int k = 0; k <= 2 * R; ++k) acc = fmaf(w[k], win[o + k], acc);
+    b[o] = acc;
+  }
+}
+
+// Both separable passes + epilogue on a staged tile.  The caller has made `in` visible to the
+// whole block (cp.async.wait_group + __syncthreads) and guarantees nobody still reads `mid`.
+// Edge tiles (EDGE) patch the diagonal into vector-filled tiles and bounds-check the outputs; the
+// fast path does neither.
+template <int R, int EPI, bool EDGE>
+__device__ __forceinline__ void tile_compute(const BlurArgs& g, const PassOffsets& c,
+                                             float* out_row, const float (&w)[2 * R + 1],
+                                             int64_t row0, int64_t col0, float* in, float* mid,
+                                             float& rmax) {
+  using G = TileGeom<R>;
+  if (EDGE && g.diag && tile_is_vec<R>(g, row0, col0)) {
+    // fused CropDiagonal on the vector path: patch the diagonal elements inside the halo'd tile
+    const int64_t lo = (row0 > col0 ? row0 : col0) - R;
+    const int64_t hi = ((row0 + TTH < col0 + TTW) ? row0 + TTH : col0 + TTW) + R;
+    if (lo < hi) {                                     // block-uniform
+      for (int64_t d = lo + threadIdx.x; d < hi; d += TTHREADS)
+        in[(d - (row0 - R)) * G::IW + (d - (col0 - R))] = g.diag[d];
+      __syncthreads();
     }
   }
+  if (c.v_in >= 0) vertical_pass<R>(w, in + c.v_in, mid + c.v_mid);
   __syncthreads();
   if (c.h_mid >= 0) {
-    float win[HSTRIP + 2 * R];
-#pragma unroll
-    for (int k = 0; k < HSTRIP + 2 * R; ++k) win[k] = mid[c.h_mid + k];
     float b[HSTRIP];
-#pragma unroll
-    for (int o = 0; o < HSTRIP; ++o) {
-      float acc = 0.0f;
-#pragma unroll
-      for (int k = 0; k <= 2 * R; ++k) acc = fmaf(w[k], win[o + k], acc);
-      b[o] = acc;
-    }
-    const int64_t j0 = col0 + c.h_c0;
-    if (EPI == EPI_STATS) {
-      float v = rmax;
-#pragma unroll
-      for (int t = 0; t < HSTRIP; ++t) v = fmaxf(v, b[t]);
-      rmax = v;
-    } else if (EPI == EPI_UPPER) {
-#pragma unroll
-      for (int q = 0; q < HSTRIP / 4; ++q)
-        *reinterpret_cast<float4*>(c.out_row + j0 + 4 * q) =
-            make_float4(b[4 * q], b[4 * q + 1], b[4 * q + 2], b[4 * q + 3]);
-      float v = rmax;
-#pragma unroll
-      for (int t = 0; t < HSTRIP; ++t) v = fmaxf(v, b[t]);
-      rmax = v;
-      // Column maxima of the tile: the lanes of this warp are its 32 rows, each holding the same 16
-      // columns.  The blurred values are non-negative, so their bit patterns order like signed
-      // integers and one REDUX.MAX per column reduces across the warp (16 instructions; the
-      // shuffle butterfly before it took ~95); lane t keeps column t and issues its atomic.
-      const int lane = threadIdx.x & 31;
-      float cm = 0.0f;
-#pragma unroll
-      for (int t = 0; t < HSTRIP; ++t) {
-        const int mx = __reduce_max_sync(0xffffffffu, __float_as_int(fmaxf(b[t], 0.0f)));
-        if (lane == t) cm = __int_as_float(mx);
-      }
-      if (lane < HSTRIP) atomic_max_nonneg(g.rowmax_out + j0 + lane, cm);
-    } else if (EPI == EPI_STORE) {
-#pragma unroll
-      for (int q = 0; q < HSTRIP / 4; ++q)
-        *reinterpret_cast<float4*>(c.out_row + j0 + 4 * q) =
-            make_float4(b[4 * q], b[4 * q + 1], b[4 * q + 2], b[4 * q + 3]);
-      if (g.rowmax_out) {
-        float v = 0.0f;
-#pragma unroll
-        for (int t = 0; t < HSTRIP; ++t) v = fmaxf(v, b[t]);
-        atomic_max_nonneg(g.rowmax_out + (c.out_row - g.out) / g.ldo + g.out_row_base, v);
-      }
-    } else {
-      float y[HSTRIP];
-#pragma unroll
-      for (int q = 0; q < HSTRIP / 4; ++q) {
-        const float4 mq = *reinterpret_cast<const float4*>(g.m + j0 + 4 * q);   // warp-broadcast
-        const float mj[4] = {mq.x, mq.y, mq.z, mq.w};
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const float x = b[4 * q + t];
-          const float keep = g.binarize ? 1.0f : x;
-          const float small = x * g.mult;
-          const float t1 = (x < c.cut_i) ? small : keep;
-          const float t2 = (x < mj[t] * g.p) ? small : keep;
-          y[4 * q + t] = (g.sym_type == SC_SYMMETRIZE_MAX) ? fmaxf(t1, t2) : 0.5f * (t1 + t2);
-        }
-      }
-      if (c.y_row) {
-#pragma unroll
-        for (int q = 0; q < HSTRIP / 4; ++q)
-          *reinterpret_cast<float4*>(c.y_row + j0 + 4 * q) =
-              make_float4(y[4 * q], y[4 * q + 1], y[4 * q + 2], y[4 * q + 3]);
-      }
-      if (c.hi_row) {
-        uint32_t hw[HSTRIP / 2], lw[HSTRIP / 2];
-#pragma unroll
-        for (int q = 0; q < HSTRIP / 2; ++q) {
-          const __half2 h = __floats2half2_rn(y[2 * q], y[2 * q + 1]);
-          const float2 f = __half22float2(h);
-          const __half2 l = __floats2half2_rn(y[2 * q] - f.x, y[2 * q + 1] - f.y);
-          hw[q] = *reinterpret_cast<const uint32_t*>(&h);
-          lw[q] = *reinterpret_cast<const uint32_t*>(&l);
-        }
-        uint4* hd = reinterpret_cast<uint4*>(c.hi_row + j0);
-        uint4* ld = reinterpret_cast<uint4*>(c.lo_row + j0);
-        hd[0] = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-        hd[1] = make_uint4(hw[4], hw[5], hw[6], hw[7]);
-        ld[0] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-        ld[1] = make_uint4(lw[4], lw[5], lw[6], lw[7]);
-      }
-    }
+    horizontal_pass<R>(w, mid + c.h_mid, b);
+    const int64_t i = row0 + c.h_r, j0 = col0 + c.h_c0;
+    if (!EDGE || (i < g.row_end && j0 < g.n)) epilogue16<EPI, EDGE>(g, i, j0, b, rmax, out_row);
   }
 }
 
@@ -533,6 +469,7 @@ __device__ __forceinline__ void fast_compute(const BlurArgs& g, const FastCtx<R>
 // the two filter passes and ran latency-bound at ~28% of the roofline.
 //   EPI_STATS : row maxima of the blurred band, one register per thread, no atomics
 //   EPI_THRSYM/EPI_STORE : the band's output rows
+//   EPI_UPPER : the column tiles that touch the upper triangle: B stored, row and column maxima
 template <int R, int EPI>
 __global__ void __launch_bounds__(TTHREADS)
 k_blur_band(const BlurArgs g, const BlurWeights bw) {
@@ -566,31 +503,16 @@ k_blur_band(const BlurArgs g, const BlurWeights bw) {
     c.fill_smem[k] = on ? r * G::IW + 4 * q : -1;
     c.fill_gofs[k] = on ? (int)(r * g.lda) + 4 * q : 0;      // < 40 * lda: fits 32 bits
   }
-  {
-    const bool von = tid < G::IW * (TTH / VSTRIP);
-    const int vc = tid % G::IW, vr0 = (tid / G::IW) * VSTRIP;
-    c.v_in = von ? vr0 * G::IW + vc : -1;
-    c.v_mid = vr0 * G::MP + vc;
-    const bool hon = tid < TTH * (TTW / HSTRIP);
-    const int hr = tid % TTH;
-    c.h_c0 = (tid / TTH) * HSTRIP;
-    c.h_mid = hon ? hr * G::MP + c.h_c0 : -1;
-    const int64_t i = row0 + hr;
-    const bool row_ok = hon && i < g.row_end;
-    const int64_t io = i - g.out_row_base;
-    c.cut_i = (EPI == EPI_THRSYM && row_ok) ? g.m[i] * g.p : 0.0f;
-    c.y_row = (row_ok && g.y) ? g.y + io * g.ldy : nullptr;
-    c.hi_row = (row_ok && g.hi) ? g.hi + io * g.ldh : nullptr;
-    c.lo_row = (row_ok && g.hi) ? g.lo + io * g.ldh : nullptr;
-    c.out_row = (row_ok && g.out) ? g.out + io * g.ldo : nullptr;
-  }
+  c.pass = pass_offsets<R>(tid);
+  c.out_row = ((EPI == EPI_STORE || EPI == EPI_UPPER) && c.pass.h_mid >= 0 && row0 + c.pass.h_r < g.row_end)
+                  ? g.out + (row0 + c.pass.h_r - g.out_row_base) * g.ldo : nullptr;
   const float* band_src = g.a + (row0 - R - g.in_row_base) * g.lda - R;   // + col0 per tile
 
-  // tile_is_fast(row0, tx * TTW) for every tile of the band, reduced to four 32-bit compares per
-  // tile (the per-tile form -- a dozen 64-bit compares evaluated twice per tile by every thread --
-  // was a sixth of the kernel's instructions): the band-level
-  // conditions once, the first/last tile with a complete halo, and the run of tiles whose halo'd
-  // footprint meets the diagonal.
+  // tile_is_vec(row0, col0), the output rows inside the block and a halo'd footprint that misses
+  // the diagonal, for every tile of the band, reduced to four 32-bit compares per tile (the
+  // per-tile form -- a dozen 64-bit compares evaluated twice per tile by every thread -- was a
+  // sixth of the kernel's instructions): the band-level conditions once, the first/last tile with
+  // a complete halo, and the run of tiles whose halo'd footprint meets the diagonal.
   const bool band_fast = (row0 >= R) && (row0 + TTH + R <= g.n) && (row0 + TTH <= g.row_end) &&
                          ((g.lda & 3) == 0) && ((reinterpret_cast<uintptr_t>(g.a) & 15) == 0);
   const int tx_fast_max = (g.n >= R + TTW) ? (int)((g.n - R) / TTW) - 1 : -1;   // col0 + TTW + R <= n
@@ -620,8 +542,8 @@ k_blur_band(const BlurArgs g, const BlurWeights bw) {
     }
     __syncthreads();   // tile tx visible; everybody is out of the previous horizontal pass
     const int64_t col0 = (int64_t)tx * TTW;
-    if (is_fast(tx)) fast_compute<R, EPI>(g, c, w, col0, cur, mid, rmax);
-    else tile_compute<R, EPI>(g, w, row0, col0, cur, mid, rmax);
+    if (is_fast(tx)) tile_compute<R, EPI, false>(g, c.pass, c.out_row, w, row0, col0, cur, mid, rmax);
+    else tile_compute<R, EPI, true>(g, pass_offsets<R>(tid), nullptr, w, row0, col0, cur, mid, rmax);
   }
   if (EPI == EPI_STATS || EPI == EPI_UPPER) {
     if (threadIdx.x < TTH * (TTW / HSTRIP)) part[threadIdx.x / TTH][threadIdx.x % TTH] = rmax;
@@ -666,47 +588,9 @@ constexpr int UT = 64;
 struct UpperArgs {
   const float* b;
   int64_t n, ldb;
-  const float* m;
-  float p, mult;
-  int binarize, preserve_diag, sym_type;
-  float* y;
-  int64_t ldy;
-  __half* hi;
-  __half* lo;
-  int64_t ldh;
   int tiles;                 // ceil(n / UT)
+  RuleArgs r;
 };
-
-__device__ __forceinline__ void store_y4(const UpperArgs& g, int64_t i, int64_t j, const float (&y)[4],
-                                         bool full4) {
-  if (full4) {
-    if (g.y) *reinterpret_cast<float4*>(g.y + i * g.ldy + j) = make_float4(y[0], y[1], y[2], y[3]);
-    if (g.hi) {
-      const __half2 h0 = __floats2half2_rn(y[0], y[1]), h1 = __floats2half2_rn(y[2], y[3]);
-      *reinterpret_cast<uint2*>(g.hi + i * g.ldh + j) =
-          make_uint2(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1));
-      if (g.lo) {          // a single-MMA Diffuse reads only the hi plane
-        const float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
-        const __half2 l0 = __floats2half2_rn(y[0] - f0.x, y[1] - f0.y);
-        const __half2 l1 = __floats2half2_rn(y[2] - f1.x, y[3] - f1.y);
-        *reinterpret_cast<uint2*>(g.lo + i * g.ldh + j) =
-            make_uint2(*reinterpret_cast<const uint32_t*>(&l0), *reinterpret_cast<const uint32_t*>(&l1));
-      }
-    }
-  } else {
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      if (j + t >= g.n) continue;
-      if (g.y) g.y[i * g.ldy + j + t] = y[t];
-      if (g.hi) {
-        __half h, l;
-        split_half(y[t], h, l);
-        g.hi[i * g.ldh + j + t] = h;
-        if (g.lo) g.lo[i * g.ldh + j + t] = l;
-      }
-    }
-  }
-}
 
 // (A run-based variant -- one CTA per tile row x 8 tile columns, the next tile's loads prefetched
 // into registers -- was slower than this one-tile-per-CTA form: the extra registers cost more
@@ -715,6 +599,7 @@ __device__ __forceinline__ void store_y4(const UpperArgs& g, int64_t i, int64_t 
 __global__ void __launch_bounds__(256)
 k_thrsym_upper(const UpperArgs g) {
   __shared__ float tile[UT][UT + 1];
+  const RuleArgs& r = g.r;
   // linear index -> (TI, TJ) with TI <= TJ: row TI of the triangle starts at TI*T - TI(TI-1)/2
   const int64_t T = g.tiles, idx = blockIdx.x;
   int64_t ti = (int64_t)(((2.0 * T + 1.0) - sqrt((2.0 * T + 1.0) * (2.0 * T + 1.0) - 8.0 * (double)idx)) * 0.5);
@@ -726,20 +611,20 @@ k_thrsym_upper(const UpperArgs g) {
   const int tr = threadIdx.x >> 4, tc = (threadIdx.x & 15) * 4;
   const int64_t j = col0 + tc;
   const bool full4 = (j + 3 < g.n);
-  float mj[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+  float cut_j[4] = {0.0f, 0.0f, 0.0f, 0.0f};
   if (full4) {
-    const float4 v = *reinterpret_cast<const float4*>(g.m + j);
-    mj[0] = v.x; mj[1] = v.y; mj[2] = v.z; mj[3] = v.w;
+    const float4 v = *reinterpret_cast<const float4*>(r.m + j);
+    cut_j[0] = v.x; cut_j[1] = v.y; cut_j[2] = v.z; cut_j[3] = v.w;
   } else {
 #pragma unroll
-    for (int t = 0; t < 4; ++t) mj[t] = (j + t < g.n) ? g.m[j + t] : 0.0f;
+    for (int t = 0; t < 4; ++t) cut_j[t] = (j + t < g.n) ? r.m[j + t] : 0.0f;
   }
 #pragma unroll
-  for (int t = 0; t < 4; ++t) mj[t] *= g.p;
+  for (int t = 0; t < 4; ++t) cut_j[t] *= r.p;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    const int r = tr + 16 * k;
-    const int64_t i = row0 + r;
+    const int rr = tr + 16 * k;
+    const int64_t i = row0 + rr;
     float y[4] = {0.0f, 0.0f, 0.0f, 0.0f};
     if (i < g.n) {
       float bv[4] = {0.0f, 0.0f, 0.0f, 0.0f};
@@ -757,21 +642,14 @@ k_thrsym_upper(const UpperArgs g) {
         for (int t = 0; t < 4; ++t)
           if (j + t < i) bv[t] = g.b[(j + t) * g.ldb + i];
       }
-      const float cut_i = g.m[i] * g.p;
+      const float cut_i = r.m[i] * r.p;
+      const int64_t dcol = diag_tile ? i - j : -1;             // column of (i, i) in the run
 #pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        const float x = bv[t];
-        const float keep = g.binarize ? 1.0f : x;
-        const float small = x * g.mult;
-        const float t1 = (x < cut_i) ? small : keep;
-        const float t2 = (x < mj[t]) ? small : keep;
-        y[t] = (g.sym_type == SC_SYMMETRIZE_MAX) ? fmaxf(t1, t2) : 0.5f * (t1 + t2);
-        if (g.preserve_diag && diag_tile && i == j + t) y[t] = 1.0f;      // refinement.py:208-209
-      }
-      store_y4(g, i, j, y, full4);
+      for (int t = 0; t < 4; ++t) y[t] = thrsym_rule(r, bv[t], cut_i, cut_j[t], dcol == t);
+      store_y<4>(r, i, j, y, full4, g.n);
     }
     if (!diag_tile) {
-      tile[r][tc] = y[0]; tile[r][tc + 1] = y[1]; tile[r][tc + 2] = y[2]; tile[r][tc + 3] = y[3];
+      tile[rr][tc] = y[0]; tile[rr][tc + 1] = y[1]; tile[rr][tc + 2] = y[2]; tile[rr][tc + 3] = y[3];
     }
   }
   if (diag_tile) return;                                       // block-uniform
@@ -781,18 +659,23 @@ k_thrsym_upper(const UpperArgs g) {
   const bool full4m = (jm + 3 < g.n);
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
-    const int r = tr + 16 * k;
-    const int64_t i = col0 + r;
+    const int rr = tr + 16 * k;
+    const int64_t i = col0 + rr;
     if (i >= g.n) continue;
-    const float y[4] = {tile[tc][r], tile[tc + 1][r], tile[tc + 2][r], tile[tc + 3][r]};
-    store_y4(g, i, jm, y, full4m);
+    const float y[4] = {tile[tc][rr], tile[tc + 1][rr], tile[tc + 2][rr], tile[tc + 3][rr]};
+    store_y<4>(r, i, jm, y, full4m, g.n);
   }
 }
 
+// scipy _gaussian_kernel1d: radius = int(truncate * sigma + 0.5) with truncate = 4; sigma <= 1e-15
+// copies the input ("if sigma > 1e-15 ... else output[...] = input[...]"), i.e. radius 0.
+static int blur_radius(double sigma) { return sigma > 1e-15 ? (int)(4.0 * sigma + 0.5) : 0; }
+
+// Weights exp(-x^2/(2 sigma^2)) / sum for radius > 0 (radius 0 runs k_noblur, which takes none).
 static int make_weights(double sigma, BlurWeights& bw, int& radius) {
-  // scipy _gaussian_kernel1d: radius = int(truncate*sigma + 0.5), exp(-x^2/(2 sigma^2)) / sum
-  radius = (int)(4.0 * sigma + 0.5);
+  radius = blur_radius(sigma);
   if (radius > kMaxRadius) return 1;
+  if (radius == 0) return 0;
   double w[2 * kMaxRadius + 1], sum = 0.0;
   for (int k = -radius; k <= radius; ++k) {
     w[k + radius] = std::exp(-0.5 / (sigma * sigma) * (double)k * (double)k);
@@ -802,60 +685,47 @@ static int make_weights(double sigma, BlurWeights& bw, int& radius) {
   return 0;
 }
 
-static int check_outputs(const BlurArgs& g) {
-  SC_REQUIRE(!g.y || vec_ok_f32(g.y, g.ldy), "blur: `y` needs a 16-byte aligned base and ldy %% 4 == 0");
-  SC_REQUIRE(!g.out || vec_ok_f32(g.out, g.ldo), "blur: `out` needs a 16-byte aligned base and ldo %% 4 == 0");
-  SC_REQUIRE(!g.hi || (vec_ok_f16(g.hi, g.ldh) && vec_ok_f16(g.lo, g.ldh)),
-             "blur: the fp16 planes need 16-byte aligned bases and ldh %% 8 == 0");
-  SC_REQUIRE(!g.m || aligned16(g.m), "blur: the row-maximum vector needs a 16-byte aligned base");
+template <int EPI>
+static int launch_band(BlurArgs& g, const BlurWeights& bw, cudaStream_t st) {
+  constexpr int R = 4;
+  const size_t smem = sizeof(float) * (2 * (TTH + 2 * R) * (TTW + 2 * R) + TTH * (TTW + 2 * R + 1));
+  auto kband = k_blur_band<R, EPI>;
+  SC_CUDA(cudaFuncSetAttribute(kband, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int ntiles = (int)((g.n + TTW - 1) / TTW);
+  static int tpc_env = -1;
+  if (tpc_env < 0) {
+    const char* e = getenv("SCB_BLUR_TILES_PER_CTA");
+    tpc_env = e ? atoi(e) : 0;
+  }
+  // the upper-triangle pass uses short runs of 2 tiles (they balance the ragged band ends of the
+  // triangle); the two-pass kernels sweep runs of 4
+  g.tiles_per_cta = tpc_env > 0 ? tpc_env : (EPI == EPI_UPPER ? 2 : 4);
+  if (g.tiles_per_cta > ntiles) g.tiles_per_cta = ntiles;
+  const unsigned gy = (unsigned)((ntiles + g.tiles_per_cta - 1) / g.tiles_per_cta);
+  const dim3 grid((unsigned)((g.row_end - g.row_begin + TTH - 1) / TTH), gy);
+  kband<<<grid, TTHREADS, smem, st>>>(g, bw);
+  sc::launched();
+  SC_LAUNCH_CHECK();
   return 0;
 }
 
+// The two-pass forms (EPI_STORE / EPI_STATS / EPI_THRSYM) at any radius.
 template <int EPI>
 static int launch_blur(const sc_context* ctx, BlurArgs& g, double sigma, cudaStream_t st) {
-  if (int rc = check_outputs(g)) return rc;
-  if (sigma <= 1e-15) {     // scipy: "if sigma > 1e-15 ... else output[...] = input[...]"
-    const unsigned gy = (unsigned)std::min<int64_t>((g.n + 1023) / 1024, 64);
-    k_noblur<EPI><<<dim3((unsigned)(g.row_end - g.row_begin), gy), 256, 0, st>>>(g); sc::launched();
-    SC_LAUNCH_CHECK();
-    return 0;
-  }
+  static_assert(EPI != EPI_UPPER, "the symmetric pass launches k_blur_band directly");
+  SC_REQUIRE(g.row_end - g.row_begin <= 65535LL * 32, "sc_gaussian_blur: n too large for the tile grid");
   BlurWeights bw;
-  int radius;
-  SC_REQUIRE(make_weights(sigma, bw, radius) == 0,
+  SC_REQUIRE(make_weights(sigma, bw, g.radius) == 0,
              "sc_gaussian_blur: sigma %g needs radius > %d", sigma, kMaxRadius);
-  g.radius = radius;
-  if (radius == 0) {        // a single tap of weight 1
+  if (g.radius == 0) {      // a copy, or a single tap of weight 1
     const unsigned gy = (unsigned)std::min<int64_t>((g.n + 1023) / 1024, 64);
     k_noblur<EPI><<<dim3((unsigned)(g.row_end - g.row_begin), gy), 256, 0, st>>>(g); sc::launched();
     SC_LAUNCH_CHECK();
     return 0;
   }
-  if (radius == 4) {
-    constexpr int R = 4;
-    const size_t smem = sizeof(float) * (2 * (TTH + 2 * R) * (TTW + 2 * R) +
-                                         TTH * (TTW + 2 * R + 1));
-    auto kband = k_blur_band<R, EPI>;
-    SC_CUDA(cudaFuncSetAttribute(kband, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int ntiles = (int)((g.n + TTW - 1) / TTW);
-    static int tpc_env = -1;
-    if (tpc_env < 0) {
-      const char* e = getenv("SCB_BLUR_TILES_PER_CTA");
-      tpc_env = e ? atoi(e) : 0;
-    }
-    // the upper-triangle pass uses short runs of 2 tiles (they balance the ragged band ends of the
-    // triangle); the two-pass kernels sweep runs of 4
-    g.tiles_per_cta = tpc_env > 0 ? tpc_env : (EPI == EPI_UPPER ? 2 : 4);
-    if (g.tiles_per_cta > ntiles) g.tiles_per_cta = ntiles;
-    const unsigned gy = (unsigned)((ntiles + g.tiles_per_cta - 1) / g.tiles_per_cta);
-    const dim3 grid((unsigned)((g.row_end - g.row_begin + TTH - 1) / TTH), gy);
-    kband<<<grid, TTHREADS, smem, st>>>(g, bw);
-    sc::launched();
-    SC_LAUNCH_CHECK();
-    return 0;
-  }
-  const size_t smem = sizeof(float) * ((size_t)(GTH + 2 * radius) * (GTW + 2 * radius) +
-                                       (size_t)GTH * (GTW + 2 * radius));
+  if (g.radius == 4) return launch_band<EPI>(g, bw, st);
+  const size_t smem = sizeof(float) * ((size_t)(GTH + 2 * g.radius) * (GTW + 2 * g.radius) +
+                                       (size_t)GTH * (GTW + 2 * g.radius));
   SC_REQUIRE(smem <= ctx->smem_optin, "sc_gaussian_blur: tile needs %zu B of shared memory", smem);
   auto kern = k_blur_generic<EPI>;
   SC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -870,16 +740,23 @@ static int launch_blur(const sc_context* ctx, BlurArgs& g, double sigma, cudaStr
 
 using namespace sc;
 
-static void whole_matrix(BlurArgs& g) {
-  g.row_begin = 0; g.row_end = g.n; g.in_row_base = 0; g.out_row_base = 0;
+// Output rows [row_begin, row_end) from input rows starting at global row in_row_base.
+static BlurArgs blur_args(const float* a, int64_t n, int64_t lda, int64_t in_row_base,
+                          int64_t row_begin, int64_t row_end, const float* diag_override) {
+  BlurArgs g = {};
+  g.a = a; g.n = n; g.lda = lda; g.diag = diag_override;
+  g.row_begin = row_begin; g.row_end = row_end; g.in_row_base = in_row_base;
+  g.out_row_base = row_begin;
+  return g;
 }
 
 static int check_block(int64_t n, int64_t in_row_base, int64_t in_rows, int64_t row_begin,
-                       int64_t row_end, int radius) {
+                       int64_t row_end, double sigma) {
   SC_REQUIRE(0 <= row_begin && row_begin < row_end && row_end <= n, "blur block: bad row range");
   SC_REQUIRE((row_end - row_begin) % 32 == 0 || row_end == n,
              "blur block: the row count must be a multiple of 32 unless the block ends the matrix");
   // every input row the block can touch (after reflection at the matrix edges) must be resident
+  const int radius = blur_radius(sigma);
   const int64_t need_lo = row_begin - radius < 0 ? 0 : row_begin - radius;
   const int64_t need_hi = row_end + radius > n ? n : row_end + radius;
   SC_REQUIRE(in_row_base <= need_lo && in_row_base + in_rows >= need_hi,
@@ -889,30 +766,86 @@ static int check_block(int64_t n, int64_t in_row_base, int64_t in_rows, int64_t 
   return 0;
 }
 
+// The rule and the Y outputs of the three threshold/symmetrize entries (`lo` may be NULL here).
+static int rule_args(const char* who, const float* rowmax, double p, double mult, int binarize,
+                     int preserve_diagonal, int sym_type, float* y, int64_t ldy, void* hi,
+                     void* lo, int64_t ldh, RuleArgs& r) {
+  SC_REQUIRE(y || hi, "%s: no output given", who);
+  SC_REQUIRE(hi || !lo, "%s: a lo plane needs its hi plane", who);
+  SC_REQUIRE(sym_type == SC_SYMMETRIZE_MAX || sym_type == SC_SYMMETRIZE_AVERAGE,
+             "Unsupported symmetrize_type.");
+  SC_REQUIRE(aligned16(rowmax), "%s: the row-maximum vector needs a 16-byte aligned base", who);
+  SC_REQUIRE(!y || vec_ok_f32(y, ldy), "%s: `y` needs a 16-byte aligned base and ldy %% 4 == 0", who);
+  SC_REQUIRE(!hi || (vec_ok_f16(hi, ldh) && (!lo || vec_ok_f16(lo, ldh))),
+             "%s: the fp16 planes need 16-byte aligned bases and ldh %% 8 == 0", who);
+  r = RuleArgs{rowmax, (float)p, (float)mult, binarize, preserve_diagonal, sym_type,
+               y, ldy, (__half*)hi, (__half*)lo, ldh};
+  return 0;
+}
+
 extern "C" int sc_gaussian_blur(sc_context* ctx, const float* a, int64_t n, int64_t lda,
                                 const float* diag_override, double sigma, float* out,
                                 int64_t ldo, float* rowmax_out, void* stream) {
   SC_REQUIRE(ctx && a && n > 0, "sc_gaussian_blur: bad arguments");
   SC_REQUIRE(out || rowmax_out, "sc_gaussian_blur: nothing to compute");
-  SC_REQUIRE(n <= 65535LL * 32, "sc_gaussian_blur: n too large for the tile grid");
-  BlurArgs g = {};
-  g.a = a; g.n = n; g.lda = lda; g.diag = diag_override;
+  SC_REQUIRE(!out || vec_ok_f32(out, ldo), "blur: `out` needs a 16-byte aligned base and ldo %% 4 == 0");
+  BlurArgs g = blur_args(a, n, lda, 0, 0, n, diag_override);
   g.out = out; g.ldo = ldo; g.rowmax_out = rowmax_out;
-  whole_matrix(g);
   if (out) return launch_blur<EPI_STORE>(ctx, g, sigma, as_stream(stream));
   return launch_blur<EPI_STATS>(ctx, g, sigma, as_stream(stream));
+}
+
+// ---- row blocks (multi-GPU row sharding, SURVEY.md 8(e)): `a` holds global rows
+// [in_row_base, in_row_base + in_rows) -- the owned rows plus the blur halo, recomputed locally
+// from the embeddings instead of exchanged; outputs cover global rows [row_begin, row_end) and are
+// written to buffers whose row 0 is global row `row_begin`.  diag_override / rowmax vectors are
+// indexed by global row.  The whole-matrix entries are the block [0, n) with the input at row 0.
+static int blur_rowmax_rows(const char* who, sc_context* ctx, const float* a, int64_t n,
+                            int64_t lda, int64_t in_row_base, int64_t in_rows, int64_t row_begin,
+                            int64_t row_end, const float* diag_override, double sigma,
+                            int zero_diagonal, float* rowmax_out, void* stream) {
+  SC_REQUIRE(ctx && a && rowmax_out && n > 0, "%s: bad arguments", who);
+  if (int rc = check_block(n, in_row_base, in_rows, row_begin, row_end, sigma)) return rc;
+  BlurArgs g = blur_args(a, n, lda, in_row_base, row_begin, row_end, diag_override);
+  g.rowmax_out = rowmax_out; g.stats_zero_diag = zero_diagonal;
+  return launch_blur<EPI_STATS>(ctx, g, sigma, as_stream(stream));
+}
+
+static int blur_thrsym_rows(const char* who, sc_context* ctx, const float* a, int64_t n,
+                            int64_t lda, int64_t in_row_base, int64_t in_rows, int64_t row_begin,
+                            int64_t row_end, const float* diag_override, double sigma,
+                            const float* rowmax, double p, double mult, int binarize,
+                            int preserve_diagonal, int sym_type, float* y, int64_t ldy, void* hi,
+                            void* lo, int64_t ldh, void* stream) {
+  SC_REQUIRE(ctx && a && rowmax && n > 0, "%s: bad arguments", who);
+  SC_REQUIRE((hi == nullptr) == (lo == nullptr), "hi/lo must come together");
+  RuleArgs r;
+  if (int rc = rule_args(who, rowmax, p, mult, binarize, preserve_diagonal, sym_type, y, ldy, hi,
+                         lo, ldh, r))
+    return rc;
+  if (int rc = check_block(n, in_row_base, in_rows, row_begin, row_end, sigma)) return rc;
+  BlurArgs g = blur_args(a, n, lda, in_row_base, row_begin, row_end, diag_override);
+  g.r = r;
+  return launch_blur<EPI_THRSYM>(ctx, g, sigma, as_stream(stream));
 }
 
 // statistics pass with the diagonal read as zero (RowWiseThreshold preserve_diagonal)
 extern "C" int sc_gaussian_blur_rowmax(sc_context* ctx, const float* a, int64_t n, int64_t lda,
                                        const float* diag_override, double sigma,
                                        int zero_diagonal, float* rowmax_out, void* stream) {
-  SC_REQUIRE(ctx && a && rowmax_out && n > 0, "sc_gaussian_blur_rowmax: bad arguments");
-  BlurArgs g = {};
-  g.a = a; g.n = n; g.lda = lda; g.diag = diag_override;
-  g.rowmax_out = rowmax_out; g.stats_zero_diag = zero_diagonal;
-  whole_matrix(g);
-  return launch_blur<EPI_STATS>(ctx, g, sigma, as_stream(stream));
+  return blur_rowmax_rows("sc_gaussian_blur_rowmax", ctx, a, n, lda, 0, n, 0, n, diag_override,
+                          sigma, zero_diagonal, rowmax_out, stream);
+}
+
+extern "C" int sc_gaussian_blur_rowmax_block(sc_context* ctx, const float* a, int64_t n,
+                                             int64_t lda, int64_t in_row_base, int64_t in_rows,
+                                             int64_t row_begin, int64_t row_end,
+                                             const float* diag_override, double sigma,
+                                             int zero_diagonal, float* rowmax_out,
+                                             void* stream) {
+  return blur_rowmax_rows("sc_gaussian_blur_rowmax_block", ctx, a, n, lda, in_row_base, in_rows,
+                          row_begin, row_end, diag_override, sigma, zero_diagonal, rowmax_out,
+                          stream);
 }
 
 extern "C" int sc_blur_threshold_symmetrize(sc_context* ctx, const float* a, int64_t n,
@@ -921,40 +854,9 @@ extern "C" int sc_blur_threshold_symmetrize(sc_context* ctx, const float* a, int
                                             double mult, int binarize, int preserve_diagonal,
                                             int sym_type, float* y, int64_t ldy, void* hi,
                                             void* lo, int64_t ldh, void* stream) {
-  SC_REQUIRE(ctx && a && rowmax && n > 0, "sc_blur_threshold_symmetrize: bad arguments");
-  SC_REQUIRE(y || (hi && lo), "sc_blur_threshold_symmetrize: no output given");
-  SC_REQUIRE((hi == nullptr) == (lo == nullptr), "hi/lo must come together");
-  SC_REQUIRE(sym_type == SC_SYMMETRIZE_MAX || sym_type == SC_SYMMETRIZE_AVERAGE,
-             "Unsupported symmetrize_type.");
-  BlurArgs g = {};
-  g.a = a; g.n = n; g.lda = lda; g.diag = diag_override;
-  g.m = rowmax; g.p = (float)p; g.mult = (float)mult; g.binarize = binarize;
-  g.preserve_diag = preserve_diagonal; g.sym_type = sym_type;
-  g.y = y; g.ldy = ldy; g.hi = (__half*)hi; g.lo = (__half*)lo; g.ldh = ldh;
-  whole_matrix(g);
-  return launch_blur<EPI_THRSYM>(ctx, g, sigma, as_stream(stream));
-}
-
-// ---- row-block variants (multi-GPU row sharding, SURVEY.md 8(e)): `a` holds global rows
-// [in_row_base, in_row_base + in_rows) -- the owned rows plus the blur halo, recomputed locally
-// from the embeddings instead of exchanged; outputs cover global rows [row_begin, row_end) and are
-// written to buffers whose row 0 is global row `row_begin`.  diag_override / rowmax vectors are
-// indexed by global row.
-extern "C" int sc_gaussian_blur_rowmax_block(sc_context* ctx, const float* a, int64_t n,
-                                             int64_t lda, int64_t in_row_base, int64_t in_rows,
-                                             int64_t row_begin, int64_t row_end,
-                                             const float* diag_override, double sigma,
-                                             int zero_diagonal, float* rowmax_out,
-                                             void* stream) {
-  SC_REQUIRE(ctx && a && rowmax_out && n > 0, "sc_gaussian_blur_rowmax_block: bad arguments");
-  const int radius = sigma > 1e-15 ? (int)(4.0 * sigma + 0.5) : 0;
-  if (int rc = check_block(n, in_row_base, in_rows, row_begin, row_end, radius)) return rc;
-  BlurArgs g = {};
-  g.a = a; g.n = n; g.lda = lda; g.diag = diag_override;
-  g.rowmax_out = rowmax_out; g.stats_zero_diag = zero_diagonal;
-  g.row_begin = row_begin; g.row_end = row_end; g.in_row_base = in_row_base;
-  g.out_row_base = row_begin;
-  return launch_blur<EPI_STATS>(ctx, g, sigma, as_stream(stream));
+  return blur_thrsym_rows("sc_blur_threshold_symmetrize", ctx, a, n, lda, 0, n, 0, n,
+                          diag_override, sigma, rowmax, p, mult, binarize, preserve_diagonal,
+                          sym_type, y, ldy, hi, lo, ldh, stream);
 }
 
 extern "C" int sc_blur_threshold_symmetrize_block(
@@ -962,21 +864,9 @@ extern "C" int sc_blur_threshold_symmetrize_block(
     int64_t row_begin, int64_t row_end, const float* diag_override, double sigma,
     const float* rowmax, double p, double mult, int binarize, int preserve_diagonal, int sym_type,
     float* y, int64_t ldy, void* hi, void* lo, int64_t ldh, void* stream) {
-  SC_REQUIRE(ctx && a && rowmax && n > 0, "sc_blur_threshold_symmetrize_block: bad arguments");
-  SC_REQUIRE(y || (hi && lo), "sc_blur_threshold_symmetrize_block: no output given");
-  SC_REQUIRE((hi == nullptr) == (lo == nullptr), "hi/lo must come together");
-  SC_REQUIRE(sym_type == SC_SYMMETRIZE_MAX || sym_type == SC_SYMMETRIZE_AVERAGE,
-             "Unsupported symmetrize_type.");
-  const int radius = sigma > 1e-15 ? (int)(4.0 * sigma + 0.5) : 0;
-  if (int rc = check_block(n, in_row_base, in_rows, row_begin, row_end, radius)) return rc;
-  BlurArgs g = {};
-  g.a = a; g.n = n; g.lda = lda; g.diag = diag_override;
-  g.m = rowmax; g.p = (float)p; g.mult = (float)mult; g.binarize = binarize;
-  g.preserve_diag = preserve_diagonal; g.sym_type = sym_type;
-  g.y = y; g.ldy = ldy; g.hi = (__half*)hi; g.lo = (__half*)lo; g.ldh = ldh;
-  g.row_begin = row_begin; g.row_end = row_end; g.in_row_base = in_row_base;
-  g.out_row_base = row_begin;
-  return launch_blur<EPI_THRSYM>(ctx, g, sigma, as_stream(stream));
+  return blur_thrsym_rows("sc_blur_threshold_symmetrize_block", ctx, a, n, lda, in_row_base,
+                          in_rows, row_begin, row_end, diag_override, sigma, rowmax, p, mult,
+                          binarize, preserve_diagonal, sym_type, y, ldy, hi, lo, ldh, stream);
 }
 
 // ---- symmetric whole-matrix pair (single-GPU hot path).  Pass 1: b_out <- the tiles of blur(a)
@@ -988,15 +878,16 @@ extern "C" int sc_blur_upper_rowmax(sc_context* ctx, const float* a, int64_t n, 
                                     const float* diag_override, double sigma, int zero_diagonal,
                                     float* b_out, int64_t ldb, float* rowmax_out, void* stream) {
   SC_REQUIRE(ctx && a && b_out && rowmax_out && n > 0, "sc_blur_upper_rowmax: bad arguments");
-  SC_REQUIRE(sigma > 1e-15 && (int)(4.0 * sigma + 0.5) == 4,
+  SC_REQUIRE(blur_radius(sigma) == 4,
              "sc_blur_upper_rowmax: the symmetric pass is built for radius 4 (sigma ~ 1)");
   SC_REQUIRE(n <= 65535LL * 32, "sc_blur_upper_rowmax: n too large for the tile grid");
-  BlurArgs g = {};
-  g.a = a; g.n = n; g.lda = lda; g.diag = diag_override;
+  SC_REQUIRE(vec_ok_f32(b_out, ldb), "blur: `out` needs a 16-byte aligned base and ldo %% 4 == 0");
+  BlurArgs g = blur_args(a, n, lda, 0, 0, n, diag_override);
   g.out = b_out; g.ldo = ldb; g.rowmax_out = rowmax_out; g.stats_zero_diag = zero_diagonal;
-  whole_matrix(g);
+  BlurWeights bw;
+  make_weights(sigma, bw, g.radius);
   SC_CUDA(cudaMemsetAsync(rowmax_out, 0, sizeof(float) * n, as_stream(stream)));
-  return launch_blur<EPI_UPPER>(ctx, g, sigma, as_stream(stream));
+  return launch_band<EPI_UPPER>(g, bw, as_stream(stream));
 }
 
 // Pass 2: y / planes <- sym(thr(b, m_i), thr(b, m_j)) for the WHOLE matrix from the upper tiles of b.
@@ -1006,17 +897,12 @@ extern "C" int sc_threshold_symmetrize_upper(sc_context* ctx, const float* b, in
                                              float* y, int64_t ldy, void* hi, void* lo, int64_t ldh,
                                              void* stream) {
   SC_REQUIRE(ctx && b && rowmax && n > 0, "sc_threshold_symmetrize_upper: bad arguments");
-  SC_REQUIRE(y || hi, "sc_threshold_symmetrize_upper: no output given");
-  SC_REQUIRE(hi || !lo, "sc_threshold_symmetrize_upper: a lo plane needs its hi plane");
-  SC_REQUIRE(sym_type == SC_SYMMETRIZE_MAX || sym_type == SC_SYMMETRIZE_AVERAGE,
-             "Unsupported symmetrize_type.");
-  SC_REQUIRE(vec_ok_f32(b, ldb) && aligned16(rowmax), "sc_threshold_symmetrize_upper: `b` / rowmax alignment");
   UpperArgs g = {};
-  g.b = b; g.n = n; g.ldb = ldb; g.m = rowmax; g.p = (float)p; g.mult = (float)mult;
-  g.binarize = binarize; g.preserve_diag = preserve_diagonal; g.sym_type = sym_type;
-  g.y = y; g.ldy = ldy; g.hi = (__half*)hi; g.lo = (__half*)lo; g.ldh = ldh;
-  SC_REQUIRE(!y || vec_ok_f32(y, ldy), "sc_threshold_symmetrize_upper: `y` alignment");
-  SC_REQUIRE(!hi || (vec_ok_f16(hi, ldh) && (!lo || vec_ok_f16(lo, ldh))), "sc_threshold_symmetrize_upper: plane alignment");
+  if (int rc = rule_args("sc_threshold_symmetrize_upper", rowmax, p, mult, binarize,
+                         preserve_diagonal, sym_type, y, ldy, hi, lo, ldh, g.r))
+    return rc;
+  SC_REQUIRE(vec_ok_f32(b, ldb), "sc_threshold_symmetrize_upper: `b` alignment");
+  g.b = b; g.n = n; g.ldb = ldb;
   g.tiles = (int)((n + UT - 1) / UT);
   const int64_t pairs = (int64_t)g.tiles * (g.tiles + 1) / 2;
   SC_REQUIRE(pairs < (1LL << 31), "sc_threshold_symmetrize_upper: n too large for the tile grid");

@@ -45,6 +45,12 @@ def round_up(x: int, m: int) -> int:
   return (x + m - 1) // m * m
 
 
+def blur_radius(sigma: float) -> int:
+  """scipy.ndimage.gaussian_filter's radius int(truncate * sigma + 0.5), truncate = 4; sigma <=
+  1e-15 copies the input (radius 0).  The blur kernels apply the same rule."""
+  return int(4.0 * sigma + 0.5) if sigma > 1e-15 else 0
+
+
 class Engine:
   """One per CUDA device: the sc_context plus allocation / launch helpers."""
 
@@ -277,7 +283,7 @@ class Engine:
   @staticmethod
   def upper_pass_ok(sigma: float) -> bool:
     """The symmetric blur pair covers radius-4 filters (sigma ~ 1, every BASELINE config)."""
-    return sigma > 1e-15 and int(4.0 * sigma + 0.5) == 4
+    return blur_radius(sigma) == 4
 
   def split_planes(self, a, n):
     hi, lo = self.planes(n)

@@ -126,10 +126,6 @@ class _Once:
       self.done = True
 
 
-def blur_radius(sigma: float) -> int:
-  return int(4.0 * sigma + 0.5) if sigma > 1e-15 else 0
-
-
 class ShardedRefiner:
   """[CropDiagonal] [GaussianBlur] RowWiseThreshold(RowMax) Symmetrize Diffuse on row blocks.
 
@@ -191,6 +187,7 @@ class ShardedRefiner:
     return [works[-1]] * len(recvs), works
 
   def run(self, embeddings, world: int = 1, rank: int = 0):
+    from .device import blur_radius
     be, opt = self.backend, self.options
     n = int(embeddings.shape[0])
     plan = ShardPlan(n, world, rank, blur_radius(self.sigma))
