@@ -357,6 +357,18 @@ int sc_cosine_distances_f64(sc_context* ctx, const void* x, int x_is_f64, int64_
 int sc_complete_linkage(sc_context* ctx, double* dist, int64_t n, int64_t ldd, int64_t* merge_xy,
                         double* merge_dist, int64_t* merge_size, void* stream);
 
+/* ---- AgglomerativeClustering(metric="cosine", linkage="average", distance_threshold=t) -------
+ * The single-cluster check of SingleClusterCondition.FallbackClusterer with
+ * FallbackClustererType.Agglomerative (fallback_clusterer.py:179-184) inside predict().  The
+ * distances come from sc_cosine_distances_f64; the threshold cut is host logic.
+ *
+ * Average-linkage NN-chain: the same arguments, chain rules, outputs and contract as
+ * sc_complete_linkage, except for the update after a merge of x < y with nx, ny points:
+ * dist[y,i] = dist[i,y] = (nx dist[x,i] + ny dist[y,i]) / (nx + ny), each product, the sum and the
+ * quotient rounded to nearest in turn (scipy's _average, no fused multiply-add).  SYNCHRONOUS. */
+int sc_average_linkage(sc_context* ctx, double* dist, int64_t n, int64_t ldd, int64_t* merge_xy,
+                       double* merge_dist, int64_t* merge_size, void* stream);
+
 /* ---- fallback_clusterer.check_single_cluster, AffinityGmmBic (fallback_clusterer.py:158-178) --
  * scikit-learn's GaussianMixture(1) and (2) fitted to affinity[np.triu_indices(n, offset)], as
  * one streaming reduction per step; the KMeans / EM / BIC control flow is host logic

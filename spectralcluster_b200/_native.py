@@ -96,6 +96,7 @@ PROTOTYPES = {
     "sc_cosine_distances_f64": [c_ptr, c_ptr, c_int, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr,
                                 c_ptr],
     "sc_complete_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_average_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_gmm_band_pass": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_int, c_ptr, c_ptr, c_ptr, c_ptr],
 }
 

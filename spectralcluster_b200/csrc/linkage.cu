@@ -1,12 +1,13 @@
-// Complete-linkage cosine agglomerative clustering (scikit-learn AgglomerativeClustering(
-// metric="cosine", linkage="complete") = scipy pdist(x, "cosine") + scipy linkage(..., "complete")):
+// Complete- and average-linkage cosine agglomerative clustering (scikit-learn
+// AgglomerativeClustering(metric="cosine", linkage="complete" / "average") = scipy pdist(x,
+// "cosine") + scipy linkage(..., "complete" / "average")):
 //   k_row_norms        |x_i| in fp64, one thread per row
 //   k_cosine_dist      D = 1 - clamp(X X^T / (|x_i| |x_j|), -1, 1), fp64 tensor cores, upper 64x64
 //                      tiles only, each tile stored and mirror-stored through shared memory
-//   k_nn_chain         scipy's nn_chain, every merge in one cooperative launch: each chain step is
+//   k_nn_chain<L>      scipy's nn_chain, every merge in one cooperative launch: each chain step is
 //                      a row scan split across the grid (one CTA per SM), a grid barrier, and a
 //                      redundant reduction of the per-CTA minima in every CTA; a merge adds a
-//                      row + column update and one more barrier.
+//                      row + column update (the linkage's Lance-Williams rule) and one more barrier.
 #include "common.cuh"
 
 #include <climits>
@@ -129,9 +130,12 @@ __device__ __forceinline__ void warp_min_idx(double& v, int& i) {
   }
 }
 
+enum class Linkage { Complete, Average };
+
 // Every CTA runs the same chain bookkeeping on the same reduced values, so all agree on every
 // decision without a broadcast.  D and size change inside the launch: they are read with
 // ld.global.cg (L2, never a stale L1 line) and written with st.global.cg.
+template <Linkage L>
 __global__ void __launch_bounds__(NN_THREADS)
 k_nn_chain(double* __restrict__ dist, int64_t n, int64_t ldd, int* __restrict__ size,
            int* __restrict__ chain, double* __restrict__ part_v, int* __restrict__ part_i,
@@ -155,6 +159,15 @@ k_nn_chain(double* __restrict__ dist, int64_t n, int64_t ldd, int* __restrict__ 
       while (__ldcg(size + lo) == 0) ++lo;
       x = lo, prev = -1, len = 1;
       if (threadIdx.x == 0) __stcg(chain, x);
+    }
+    // A merge in this step joins x and prev.  Average linkage weighs their rows by their sizes,
+    // which CTA 0 rewrites in the merge phase while other CTAs may still update; so every thread
+    // reads both sizes here.  The last size writes were fenced by the previous merge's barrier and
+    // the next ones follow this step's barrier: no write can overlap these loads.
+    int nx = 0, nprev = 0;
+    if constexpr (L == Linkage::Average) {
+      nx = __ldcg(size + x);
+      nprev = prev >= 0 ? __ldcg(size + prev) : 0;
     }
     // ---- nearest active neighbour of x in this CTA's columns
     const double* row = dist + (int64_t)x * ldd;
@@ -205,11 +218,27 @@ k_nn_chain(double* __restrict__ dist, int64_t n, int64_t ldd, int* __restrict__ 
     const int a = x < y ? x : y, b = x < y ? y : x;
     const double* ra = dist + (int64_t)a * ldd;
     double* rb = dist + (int64_t)b * ldd;
-    for (int64_t i = beg + threadIdx.x; i < end; i += NN_THREADS) {
-      if (i == a || i == b || __ldcg(size + i) == 0) continue;
-      const double v = fmax(__ldcg(ra + i), __ldcg(rb + i));
-      __stcg(rb + i, v);
-      __stcg(dist + i * ldd + b, v);
+    if constexpr (L == Linkage::Complete) {
+      for (int64_t i = beg + threadIdx.x; i < end; i += NN_THREADS) {
+        if (i == a || i == b || __ldcg(size + i) == 0) continue;
+        const double v = fmax(__ldcg(ra + i), __ldcg(rb + i));
+        __stcg(rb + i, v);
+        __stcg(dist + i * ldd + b, v);
+      }
+    } else {
+      const double na = a == x ? nx : nprev, nb = a == x ? nprev : nx, nab = nx + nprev;
+      // not unrolled: the division's slow path is a subroutine call, and the values an unrolled
+      // loop keeps live across it spill
+#pragma unroll 1
+      for (int64_t i = beg + threadIdx.x; i < end; i += NN_THREADS) {
+        if (i == a || i == b || __ldcg(size + i) == 0) continue;
+        // scipy's _average, (na d_ai + nb d_bi) / (na + nb), rounded step by step: a contracted
+        // FMA would round once less and break bitwise equality with scipy
+        const double v = __ddiv_rn(
+            __dadd_rn(__dmul_rn(na, __ldcg(ra + i)), __dmul_rn(nb, __ldcg(rb + i))), nab);
+        __stcg(rb + i, v);
+        __stcg(dist + i * ldd + b, v);
+      }
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) {   // no CTA reads size[a] or size[b] in this phase
       const int sz = __ldcg(size + a) + __ldcg(size + b);
@@ -254,15 +283,17 @@ extern "C" int sc_cosine_distances_f64(sc_context* ctx, const void* x, int x_is_
   return 0;
 }
 
-extern "C" int sc_complete_linkage(sc_context* ctx, double* dist, int64_t n, int64_t ldd,
-                                   int64_t* merge_xy, double* merge_dist, int64_t* merge_size,
-                                   void* stream) {
+namespace {
+
+template <Linkage L>
+int nn_chain_linkage(const char* name, sc_context* ctx, double* dist, int64_t n, int64_t ldd,
+                     int64_t* merge_xy, double* merge_dist, int64_t* merge_size, void* stream) {
   SC_REQUIRE(ctx && dist && merge_xy && merge_dist && merge_size && n >= 2 && n < INT_MAX &&
-             ldd >= n, "sc_complete_linkage: bad arguments");
+             ldd >= n, "%s: bad arguments", name);
   cudaStream_t st = as_stream(stream);
   int per_sm = 0;
-  SC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_nn_chain, NN_THREADS, 0));
-  SC_REQUIRE(per_sm >= 1, "sc_complete_linkage: the NN-chain kernel does not fit on an SM");
+  SC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_nn_chain<L>, NN_THREADS, 0));
+  SC_REQUIRE(per_sm >= 1, "%s: the NN-chain kernel does not fit on an SM", name);
   // one CTA per SM: every CTA takes part in every grid barrier and reduces every partial, so
   // more CTAs would only add barrier and reduction work to an O(n) scan
   const int64_t want = (n + NN_THREADS - 1) / NN_THREADS;
@@ -288,7 +319,7 @@ extern "C" int sc_complete_linkage(sc_context* ctx, double* dist, int64_t n, int
   double* md_ = md.as<double>();
   int64_t* ms_ = ms.as<int64_t>();
   void* args[] = {&d_, &n_, &ldd_, &size_, &chain_, &pv_, &pi_, &xy_, &md_, &ms_};
-  SC_CUDA(cudaLaunchCooperativeKernel((const void*)k_nn_chain, dim3((unsigned)grid),
+  SC_CUDA(cudaLaunchCooperativeKernel((const void*)k_nn_chain<L>, dim3((unsigned)grid),
                                       dim3(NN_THREADS), args, 0, st));
   launched(2);
   SC_CUDA(cudaMemcpyAsync(merge_xy, xy_, sizeof(int64_t) * 2 * m, cudaMemcpyDeviceToHost, st));
@@ -296,4 +327,20 @@ extern "C" int sc_complete_linkage(sc_context* ctx, double* dist, int64_t n, int
   SC_CUDA(cudaMemcpyAsync(merge_size, ms_, sizeof(int64_t) * m, cudaMemcpyDeviceToHost, st));
   SC_CUDA(cudaStreamSynchronize(st));
   return 0;
+}
+
+}  // namespace
+
+extern "C" int sc_complete_linkage(sc_context* ctx, double* dist, int64_t n, int64_t ldd,
+                                   int64_t* merge_xy, double* merge_dist, int64_t* merge_size,
+                                   void* stream) {
+  return nn_chain_linkage<Linkage::Complete>("sc_complete_linkage", ctx, dist, n, ldd, merge_xy,
+                                             merge_dist, merge_size, stream);
+}
+
+extern "C" int sc_average_linkage(sc_context* ctx, double* dist, int64_t n, int64_t ldd,
+                                  int64_t* merge_xy, double* merge_dist, int64_t* merge_size,
+                                  void* stream) {
+  return nn_chain_linkage<Linkage::Average>("sc_average_linkage", ctx, dist, n, ldd, merge_xy,
+                                            merge_dist, merge_size, stream);
 }

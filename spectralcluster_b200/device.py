@@ -145,8 +145,9 @@ class Engine:
       "sc_affinity_stats": "fallback_clusterer.check_single_cluster",
       "sc_gmm_band_pass": "fallback_clusterer.check_single_cluster",
       "sc_constraint_combine": "constraint.adjust_affinity", "sc_scale_shift": "constraint.adjust_affinity",
-      "sc_cosine_distances_f64": "AgglomerativeClustering(cosine, complete)",
+      "sc_cosine_distances_f64": "AgglomerativeClustering(cosine)",
       "sc_complete_linkage": "AgglomerativeClustering(cosine, complete)",
+      "sc_average_linkage": "AgglomerativeClustering(cosine, average)",
   }
   nvtx = os.environ.get("SCB_NVTX") == "1"
 
@@ -412,12 +413,19 @@ class Engine:
   def complete_linkage(self, dist, n: int):
     """Complete-linkage NN-chain over the device distance matrix (overwritten) -> host
     (xy int64 [n-1, 2], distance fp64 [n-1], size int64 [n-1]), in chain order."""
+    return self._nn_chain("sc_complete_linkage", dist, n)
+
+  def average_linkage(self, dist, n: int):
+    """Average-linkage NN-chain over the device distance matrix (overwritten) -> host
+    (xy int64 [n-1, 2], distance fp64 [n-1], size int64 [n-1]), in chain order."""
+    return self._nn_chain("sc_average_linkage", dist, n)
+
+  def _nn_chain(self, entry, dist, n: int):
     xy = np.empty((n - 1, 2), dtype=np.int64)
     md = np.empty(n - 1, dtype=np.float64)
     ms = np.empty(n - 1, dtype=np.int64)
-    self.call("sc_complete_linkage", _ptr(dist), n, dist.stride(0),
-              xy.ctypes.data_as(ctypes.c_void_p), md.ctypes.data_as(ctypes.c_void_p),
-              ms.ctypes.data_as(ctypes.c_void_p), self.stream)
+    self.call(entry, _ptr(dist), n, dist.stride(0), xy.ctypes.data_as(ctypes.c_void_p),
+              md.ctypes.data_as(ctypes.c_void_p), ms.ctypes.data_as(ctypes.c_void_p), self.stream)
     return xy, md, ms
 
 

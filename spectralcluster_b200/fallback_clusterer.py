@@ -9,8 +9,11 @@ What runs where:
     device for a device-resident affinity, one streaming pass per KMeans / EM step
     (`gmm_bic`, `sc_gmm_band_pass`), with scikit-learn's arithmetic and random draws; a host
     ndarray still goes to scikit-learn;
-  * FallbackClusterer (scikit-learn average-linkage AHC, or the sequential naive clusterer) only
-    ever sees inputs below `spectral_min_embeddings` or acts as a probe: host.
+  * FallbackClusterer as the probe of predict(), Agglomerative type: average-linkage cosine AHC
+    on the device with scikit-learn's cluster count (agglomerative.CosineAverageLinkage); a host
+    ndarray affinity still goes to scikit-learn;
+  * FallbackClusterer otherwise (inputs below `spectral_min_embeddings`, the sequential naive
+    clusterer, FallbackClusterer.predict): host.
 """
 
 from __future__ import annotations
@@ -92,12 +95,15 @@ def affinity_statistics(affinity) -> typing.Dict[str, float]:
 
 def check_single_cluster(fallback_options: FallbackOptions,
                          embeddings: typing.Optional[np.ndarray], affinity,
-                         details: typing.Optional[dict] = None) -> bool:
+                         details: typing.Optional[dict] = None,
+                         embeddings_dev=None) -> bool:
   """True when the data form a single cluster (only consulted when min_clusters == 1).
 
   `affinity` is a host ndarray (reference signature) or the DeviceAffinity predict() holds.
   For AffinityGmmBic on a device affinity, `details` (if given) receives the two BICs, both
-  GMMs' EM iteration counts and the number of passes over the affinity."""
+  GMMs' EM iteration counts and the number of passes over the affinity.  The Agglomerative
+  fallback clusterer on a device affinity runs on the device too, on `embeddings_dev` (the
+  embeddings as a CUDA tensor) when given and on an uploaded copy of `embeddings` otherwise."""
   cond = fallback_options.single_cluster_condition
   thr = fallback_options.single_cluster_affinity_threshold
   if cond == SingleClusterCondition.AllAffinity:
@@ -124,6 +130,12 @@ def check_single_cluster(fallback_options: FallbackOptions,
     bic = [GaussianMixture(n_components=c).fit(values).bic(values) for c in (1, 2)]
     return bool(bic[0] < bic[1])
   if cond == SingleClusterCondition.FallbackClusterer:
+    if (fallback_options.fallback_clusterer_type == FallbackClustererType.Agglomerative and
+        not isinstance(affinity, np.ndarray)):
+      from . import agglomerative
+      probe = agglomerative.CosineAverageLinkage(fallback_options.agglomerative_threshold)
+      probe.fit_predict(embeddings if embeddings_dev is None else embeddings_dev)
+      return probe.n_clusters_ == 1
     labels = FallbackClusterer(fallback_options).predict(embeddings)
     return bool(np.unique(labels).size == 1)
   raise TypeError("Unsupported single_cluster_condition")

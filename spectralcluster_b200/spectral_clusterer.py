@@ -262,6 +262,7 @@ class SpectralClusterer:
       a, crop = eng.affinity(x_dev, want_crop_vector=crop_first)
       affinity = DeviceAffinity(a, num_embeddings, crop, True)
     else:
+      x_dev = None
       host = np.asarray(self.affinity_function(embeddings))
       affinity = DeviceAffinity(eng.upload_matrix(host), num_embeddings, None,
                                 bool(np.allclose(host, host.T, rtol=1e-6, atol=1e-9)))
@@ -270,7 +271,7 @@ class SpectralClusterer:
     if self.min_clusters == 1:
       # single-vs-multi cluster decision on the resident affinity (spectral_clusterer.py:253-256)
       if fallback_clusterer.check_single_cluster(self.fallback_options, embeddings, affinity,
-                                                 single_details):
+                                                 single_details, embeddings_dev=x_dev):
         if single_details:
           self.last_details = dict(single_cluster=single_details)
         return np.array([0] * num_embeddings)
