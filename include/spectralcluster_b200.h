@@ -403,6 +403,28 @@ int sc_gmm_band_pass(sc_context* ctx, const float* a, int64_t n, int64_t lda, in
                      int mode, const double* params_host, double* work, double* out_host,
                      void* stream);
 
+/* ---- naive_clusterer.NaiveClusterer (naive_clusterer.py:59-101) ------------------------------
+ * The online clusterer over x[0..n) in one launch, and the single-cluster check of
+ * SingleClusterCondition.FallbackClusterer with FallbackClustererType.Naive
+ * (fallback_clusterer.py:179-184).  x is [n,d] fp32 (x_is_f64=0) or fp64 (=1), read as fp64.  For
+ * each embedding e in turn: cos_c = (m_c . e) / (|m_c| |e|) over the open clusters; if max cos <
+ * threshold (or none is open) cluster C opens with m_C = e, count 1; otherwise the label is the
+ * first index of the maximum, and if that cosine > adaptation_threshold, m = (m count + e) /
+ * (count + 1), each step rounded in turn (no FMA), and count += 1.  A NaN cosine ranks above every
+ * number, as np.max / np.argmax have it: it is the label and neither opens nor merges.
+ *
+ * means (fp64 [capacity, ldm]) and counts (int64 [capacity]) are DEVICE buffers whose first
+ * initial_clusters rows hold the state to continue from (0 = fresh); on return rows [0, C) hold the
+ * final state.  stop_at > 0 stops before the next embedding as soon as stop_at clusters are open.
+ * labels (DEVICE int64 [n]) receives the labels of the processed prefix; *processed_host and
+ * *clusters_host (C) are HOST values.  capacity >= initial_clusters + n always suffices; a call
+ * that would open more clusters than capacity fails.  SYNCHRONOUS. */
+int sc_naive_cluster(sc_context* ctx, const void* x, int x_is_f64, int64_t n, int64_t d, int64_t ldx,
+                     double threshold, double adaptation_threshold, int64_t stop_at, double* means,
+                     int64_t ldm, int64_t* counts, int64_t capacity, int64_t initial_clusters,
+                     int64_t* labels, int64_t* processed_host, int64_t* clusters_host,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -98,6 +98,8 @@ PROTOTYPES = {
     "sc_complete_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_average_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_gmm_band_pass": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_int, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_naive_cluster": [c_ptr, c_ptr, c_int, c_i64, c_i64, c_i64, c_dbl, c_dbl, c_i64, c_ptr,
+                         c_i64, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
 }
 
 # enum values of include/spectralcluster_b200.h

@@ -148,6 +148,7 @@ class Engine:
       "sc_cosine_distances_f64": "AgglomerativeClustering(cosine)",
       "sc_complete_linkage": "AgglomerativeClustering(cosine, complete)",
       "sc_average_linkage": "AgglomerativeClustering(cosine, average)",
+      "sc_naive_cluster": "naive_clusterer.NaiveClusterer",
   }
   nvtx = os.environ.get("SCB_NVTX") == "1"
 
@@ -419,6 +420,32 @@ class Engine:
     """Average-linkage NN-chain over the device distance matrix (overwritten) -> host
     (xy int64 [n-1, 2], distance fp64 [n-1], size int64 [n-1]), in chain order."""
     return self._nn_chain("sc_average_linkage", dist, n)
+
+  def naive_cluster(self, x_dev, threshold: float, adaptation_threshold: float, stop_at: int = 0,
+                    means=None, counts=None):
+    """NaiveClusterer over the rows of a device [n, d] fp32/fp64 tensor (row stride free, unit
+    column stride) in one launch, continuing from device means (fp64 [c0, d]) / counts (int64
+    [c0]) when given; stop_at > 0 stops once that many clusters are open.  -> (labels int64
+    device [processed], processed, clusters, means fp64 device [clusters, d], counts int64 device
+    [clusters])."""
+    t = torch()
+    n, d = int(x_dev.shape[0]), int(x_dev.shape[1])
+    c0 = 0 if means is None else int(means.shape[0])
+    grow = n if stop_at <= 0 else min(n, max(int(stop_at) - c0, 0))
+    cap = c0 + grow
+    m = t.empty((max(cap, 1), d), dtype=t.float64, device=self.device)
+    c = t.empty((max(cap, 1),), dtype=t.int64, device=self.device)
+    if c0:
+      m[:c0].copy_(means)
+      c[:c0].copy_(counts)
+    labels = t.empty((max(n, 1),), dtype=t.int64, device=self.device)
+    processed, clusters = ctypes.c_int64(), ctypes.c_int64()
+    self.call("sc_naive_cluster", _ptr(x_dev), 1 if x_dev.dtype == t.float64 else 0, n, d,
+              x_dev.stride(0), float(threshold), float(adaptation_threshold), int(stop_at),
+              _ptr(m), m.stride(0), _ptr(c), cap, c0, _ptr(labels), ctypes.byref(processed),
+              ctypes.byref(clusters), self.stream)
+    k = clusters.value
+    return labels[:processed.value], processed.value, k, m[:k], c[:k]
 
   def _nn_chain(self, entry, dist, n: int):
     xy = np.empty((n - 1, 2), dtype=np.int64)

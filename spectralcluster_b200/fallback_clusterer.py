@@ -12,8 +12,11 @@ What runs where:
   * FallbackClusterer as the probe of predict(), Agglomerative type: average-linkage cosine AHC
     on the device with scikit-learn's cluster count (agglomerative.CosineAverageLinkage); a host
     ndarray affinity still goes to scikit-learn;
-  * FallbackClusterer otherwise (inputs below `spectral_min_embeddings`, the sequential naive
-    clusterer, FallbackClusterer.predict): host.
+  * FallbackClusterer as the probe of predict(), Naive type: the naive clusterer in one device
+    launch that stops as soon as a second cluster opens (`sc_naive_cluster`); a host ndarray
+    affinity still runs the host clusterer;
+  * FallbackClusterer otherwise (inputs below `spectral_min_embeddings`,
+    FallbackClusterer.predict): host.
 """
 
 from __future__ import annotations
@@ -101,9 +104,11 @@ def check_single_cluster(fallback_options: FallbackOptions,
 
   `affinity` is a host ndarray (reference signature) or the DeviceAffinity predict() holds.
   For AffinityGmmBic on a device affinity, `details` (if given) receives the two BICs, both
-  GMMs' EM iteration counts and the number of passes over the affinity.  The Agglomerative
-  fallback clusterer on a device affinity runs on the device too, on `embeddings_dev` (the
-  embeddings as a CUDA tensor) when given and on an uploaded copy of `embeddings` otherwise."""
+  GMMs' EM iteration counts and the number of passes over the affinity.  Both fallback clusterer
+  types on a device affinity run on the device too, on `embeddings_dev` (the embeddings as a CUDA
+  tensor) when given and on an uploaded copy of `embeddings` otherwise; the Naive type stops at
+  the second cluster and records the embeddings it processed and the clusters it opened in
+  `details`."""
   cond = fallback_options.single_cluster_condition
   thr = fallback_options.single_cluster_affinity_threshold
   if cond == SingleClusterCondition.AllAffinity:
@@ -130,12 +135,28 @@ def check_single_cluster(fallback_options: FallbackOptions,
     bic = [GaussianMixture(n_components=c).fit(values).bic(values) for c in (1, 2)]
     return bool(bic[0] < bic[1])
   if cond == SingleClusterCondition.FallbackClusterer:
-    if (fallback_options.fallback_clusterer_type == FallbackClustererType.Agglomerative and
-        not isinstance(affinity, np.ndarray)):
+    kind = fallback_options.fallback_clusterer_type
+    if kind == FallbackClustererType.Agglomerative and not isinstance(affinity, np.ndarray):
       from . import agglomerative
       probe = agglomerative.CosineAverageLinkage(fallback_options.agglomerative_threshold)
       probe.fit_predict(embeddings if embeddings_dev is None else embeddings_dev)
       return probe.n_clusters_ == 1
+    if kind == FallbackClustererType.Naive and not isinstance(affinity, np.ndarray):
+      from . import device as dev
+      probe = naive_clusterer.NaiveClusterer(fallback_options.naive_threshold,
+                                             fallback_options.naive_adaptation_threshold)
+      eng = dev.Engine.get()
+      x = embeddings_dev
+      if x is None:
+        x = np.ascontiguousarray(embeddings)
+        if x.dtype not in (np.float32, np.float64):
+          x = x.astype(np.float64)
+        x = dev.torch().from_numpy(x).to(eng.device)
+      _, processed, clusters, _, _ = eng.naive_cluster(x, probe.threshold,
+                                                       probe.adaptation_threshold, stop_at=2)
+      if details is not None:
+        details.update(processed=processed, n_clusters=clusters)
+      return clusters == 1
     labels = FallbackClusterer(fallback_options).predict(embeddings)
     return bool(np.unique(labels).size == 1)
   raise TypeError("Unsupported single_cluster_condition")

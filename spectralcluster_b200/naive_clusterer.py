@@ -3,13 +3,16 @@
 fallback_clusterer.py:114-117).
 
 Strictly sequential by definition (the label of frame t depends on the centroids after frames
-0..t-1), and only ever run on inputs too small for spectral clustering
-(`spectral_min_embeddings`) or as a single-vs-multi cluster probe: host code.  State is kept as
-one [clusters, d] matrix of running means so that each step is a single matrix-vector product.
+0..t-1).  Host ndarrays run here, one matrix-vector product per embedding over the [clusters, d]
+matrix of running means.  `predict` / `fit_predict` with a CUDA tensor run the whole sequence in
+one device launch (`sc_naive_cluster`) with the same fp64 arithmetic and leave the same state, so
+that `predict_next` continues where a host run would; the single-vs-multi cluster probe of
+predict() uses that launch too (fallback_clusterer.check_single_cluster).
 """
 
 from __future__ import annotations
 
+import sys
 import typing
 
 import numpy as np
@@ -75,8 +78,40 @@ class NaiveClusterer:
       self._counts[label] = c + 1
     return label
 
-  def predict(self, embeddings: np.ndarray) -> np.ndarray:
+  def predict(self, embeddings) -> np.ndarray:
+    """Labels of the rows of `embeddings`, continuing the current state.  A CUDA tensor is read in
+    place on the device; anything else runs on the host."""
+    if _is_cuda_tensor(embeddings):
+      return self._predict_device(embeddings)
     return np.array([self.predict_next(e) for e in embeddings])
+
+  def _predict_device(self, x) -> np.ndarray:
+    from . import device as dev
+    t = dev.torch()
+    if x.ndim != 2:
+      raise ValueError("embeddings must be 2-dimensional")
+    if x.dtype not in (t.float32, t.float64):
+      x = x.to(t.float64)
+    if x.stride(1) != 1:
+      x = x.contiguous()
+    eng = dev.Engine.get(x.device.index)
+    means = counts = None
+    if self._means is not None:
+      means = t.from_numpy(self._means).to(eng.device)
+      counts = t.tensor(self._counts, dtype=t.int64, device=eng.device)
+    labels, _, k, means, counts = eng.naive_cluster(
+        x, self.threshold, self.adaptation_threshold, means=means, counts=counts)
+    if k:
+      self._means = means.cpu().numpy()
+      self._counts = counts.cpu().tolist()
+    if x.shape[0] == 0:
+      return np.array([])
+    return labels.cpu().numpy()
 
   def fit_predict(self, embeddings: np.ndarray) -> np.ndarray:
     return self.predict(embeddings)
+
+
+def _is_cuda_tensor(x) -> bool:
+  torch = sys.modules.get("torch")       # a torch tensor implies torch is imported
+  return torch is not None and isinstance(x, torch.Tensor) and x.is_cuda
