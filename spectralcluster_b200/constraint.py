@@ -8,6 +8,11 @@ Newton-Schulz iteration X <- X (2I - M X), M = I - a Abar, which starts at X = I
 a Abar (spectral radius a < 1) and squares it every step -- ceil(log2(ln 1e-9 / ln a)) steps of
 two dense products each, on the same GEMM engines as Diffuse (wgmma split-fp16 planes, or the
 SIMT fp64-accumulate engine below 64 rows).  The reference calls np.linalg.inv (:151).
+
+From X = I the iteration diverges for |a| >= 1 (the reference still inverts I - a Abar there), and
+M is held in fp32, so the error of the inverse grows with cond(M) <= (1 + |a|) / (1 - |a|).
+|a| <= MAX_ABS_ALPHA is the range measured against the float64 inverse on an H100
+(tests/test_gpu_constraint_kernels.py); any other alpha raises NotImplementedError before a launch.
 """
 
 from __future__ import annotations
@@ -24,6 +29,26 @@ from . import _native as nat
 from . import device as dev
 
 EPS = 1e-10
+# Newton-Schulz: stop once the residual's spectral radius |a|^(2^steps) is below this
+RESIDUAL_TARGET = 1e-9
+# largest |alpha| whose propagation was measured within the test tolerance on an H100 (80 GB HBM3,
+# 700 W): 0.999 stays inside it at N = 63 and 1,000; 0.9999 at N = 1,000 is 1.6x outside it
+MAX_ABS_ALPHA = 0.999
+
+
+def newton_schulz_steps(alpha: float) -> int:
+  """Steps of X <- X (2I - M X) from X = I until |alpha|^(2^steps) <= RESIDUAL_TARGET (the
+  spectral radius of the residual alpha Abar is |alpha|); raises NotImplementedError for the
+  alphas the device path does not serve."""
+  alpha = float(alpha)
+  if not abs(alpha) <= MAX_ABS_ALPHA:
+    raise NotImplementedError(
+        "ConstraintPropagation alpha={!r}: the device inverts I - alpha Abar by a Newton-Schulz "
+        "iteration, which diverges for |alpha| >= 1 and is measured accurate in fp32 only for "
+        "|alpha| <= {}".format(alpha, MAX_ABS_ALPHA))
+  if alpha == 0.0:
+    return 0                                                           # M = I: X = I is exact
+  return max(1, int(math.ceil(math.log2(math.log(RESIDUAL_TARGET) / math.log(abs(alpha))))))
 
 
 class ConstraintName(enum.Enum):
@@ -129,16 +154,17 @@ class ConstraintPropagation(ConstraintOperation):
   def __init__(self, alpha: float = 0.6):
     self.alpha = alpha
 
+  def check_input(self, affinity, constraint_matrix):
+    super().check_input(affinity, constraint_matrix)
+    newton_schulz_steps(self.alpha)
+
   def adjust_on_device(self, eng, a, q, n):
     alpha = float(self.alpha)
+    steps = newton_schulz_steps(alpha)
     _, rowsum = eng.row_stats(a, n, want_max=False, want_sum=True)
     dn = 1.0 / (dev.torch().sqrt(rowsum) + EPS)                       # :144
     m = _scale_shift(eng, a, n, -alpha, 1.0, rows=dn, cols=dn)         # M = I - alpha Abar
     x = _scale_shift(eng, m, n, 0.0, 1.0)                              # X0 = I
-    if 0.0 < abs(alpha) < 1.0:
-      steps = max(1, min(12, int(math.ceil(math.log2(math.log(1e-9) / math.log(abs(alpha)))))))
-    else:
-      steps = 12
     for _ in range(steps):                                             # X <- X (2I - M X)
       r = _scale_shift(eng, _matmul(eng, m, x, n), n, -1.0, 2.0)
       x = _matmul(eng, x, r, n)

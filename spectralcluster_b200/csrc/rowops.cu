@@ -331,7 +331,7 @@ __global__ void k_affinity_stats_finish(const double* __restrict__ part, const f
 // constraint.py:95-164.  AffinityIntegration is one element-wise pass; ConstraintPropagation is a
 // handful of dense products (host-orchestrated, on the GEMM engines) around these element-wise
 // helpers.
-//   mode 0: out = max(a, q)                       AffinityIntegration(Max)      :112-113
+//   mode 0: out = np.maximum(a, q)                AffinityIntegration(Max)      :112-113
 //   mode 1: out = (a + q) / 2                     AffinityIntegration(Average)  :114-115
 //   mode 2: out = q > 0 ? 1 - (1 - q)(1 - a) : (1 + q) a   propagation, eq. (4) :156-163
 __global__ void k_constraint_combine(const float* __restrict__ a, int64_t lda,
@@ -342,7 +342,7 @@ __global__ void k_constraint_combine(const float* __restrict__ a, int64_t lda,
   if (j >= n) return;
   const float x = a[i * lda + j], c = q[i * ldq + j];
   float r;
-  if (mode == 0) r = fmaxf(x, c);
+  if (mode == 0) r = (x >= c || x != x) ? x : c;   // np.maximum: a NaN operand propagates
   else if (mode == 1) r = 0.5f * (x + c);
   else r = (c > 0.0f) ? 1.0f - (1.0f - c) * (1.0f - x) : (1.0f + c) * x;
   out[i * ldo + j] = r;
