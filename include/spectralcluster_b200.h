@@ -265,6 +265,25 @@ int sc_eigh_extremal(sc_context* ctx, const float* s, int64_t n, int64_t lds, co
                      int64_t n_values, int64_t n_vectors, double tol, int64_t max_matvecs,
                      double* w_host, double* v_dev, int64_t* stats_host, void* stream);
 
+/* One window of a windowed extremal solve: sc_eigh_extremal restricted to the complement of the
+ * n_locked orthonormal vectors locked[0..n_locked) of the SYMMETRISED space (fp64, vector-major,
+ * stride n).  Finds the next n_values (<= 32) extremal eigenvalues of M into w_host and APPENDS
+ * their symmetrised-space Ritz vectors at locked[n_locked..n_locked+n_values) (the buffer must
+ * hold them), so the caller only advances n_locked.  A residual is converged when it is <= tol *
+ * max(largest |Ritz value|, scale): pass the magnitude of M's extremal eigenvalue once known.
+ * stats_host[4] as sc_eigh_extremal.  SYNCHRONOUS. */
+int sc_eigh_extremal_locked(sc_context* ctx, const float* s, int64_t n, int64_t lds,
+                            const double* delta, const double* left, const double* right,
+                            double sign, int which, int64_t n_values, double tol,
+                            int64_t max_matvecs, double scale, double* locked, int64_t n_locked,
+                            double* w_host, int64_t* stats_host, void* stream);
+
+/* Eigenvectors of M from symmetrised-space vectors: v_out[:, j] = E u_c / |E u_c| with
+ * c = cols_host[j], u_c = u + c * n, E = sqrt(left / right) (NULL = 1); v_out fp64 row-major
+ * [n, k].  SYNCHRONOUS. */
+int sc_eigh_mapback(sc_context* ctx, const double* u, int64_t n, const int* cols_host, int64_t k,
+                    const double* left, const double* right, double* v_out, void* stream);
+
 /* Block size b (vectors multiplied per pass over S) the extremal solver uses for n_values pairs. */
 int sc_eigh_block_size(int64_t n_values);
 

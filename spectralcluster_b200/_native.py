@@ -78,6 +78,9 @@ PROTOTYPES = {
                       c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_eigh_extremal": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_dbl, c_int, c_i64,
                          c_i64, c_dbl, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_eigh_extremal_locked": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_dbl, c_int,
+                                c_i64, c_dbl, c_i64, c_dbl, c_ptr, c_i64, c_ptr, c_ptr, c_ptr],
+    "sc_eigh_mapback": [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_eigh_block_size": [c_i64],
     "sc_eigh_extremal_sharded": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr,
                                  c_dbl, c_int, c_i64, c_i64, c_dbl, c_i64, c_ptr, c_int, c_i64,

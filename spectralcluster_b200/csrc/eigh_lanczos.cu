@@ -19,8 +19,16 @@
 //   k_proj / k_axpy_basis   the same one vector at a time, for a rank-deficient block
 //   k_combine       thick restart V <- V Z
 // The m x m projected problem (m <= 128) is solved on the host by Householder tridiagonalisation
-// and implicit QL (tred2/tql2).  The sc_krylov_* primitives at the end serve the general
-// (non-symmetric) eigen path of arnoldi.py.
+// and implicit QL (tred2/tql2).
+//
+// More pairs than one solve finds (max_clusters=None, or max_clusters >= 32, above the dense
+// solver's N) come in windows (sc_eigh_extremal_locked, driven by eigen_windows.py): each window
+// solves for the next 16 pairs of Op restricted to the complement of the pairs already found (the
+// locked set, orthogonalised out of every block with k_block_proj / k_block_axpy in chunks of
+// LOCK_CHUNK vectors: about four reads of N x L x 8 bytes per pass over S) and appends its Ritz
+// vectors to that set; sc_eigh_mapback turns the selected ones into eigenvectors of M.
+//
+// The sc_krylov_* primitives at the end serve the general (non-symmetric) eigen path of arnoldi.py.
 #include "common.cuh"
 
 #include <algorithm>
@@ -356,6 +364,7 @@ __global__ void k_combine(const double* __restrict__ v, int64_t n, int m,
 // take the same decisions).
 constexpr int BP_CHUNK = 256;      // rows per CTA
 constexpr int BP_WARPS = 8;
+constexpr int LOCK_CHUNK = 128;    // locked vectors per block projection (16 KB of coefficients)
 
 template <int B>
 __global__ void __launch_bounds__(BP_WARPS * 32)
@@ -497,13 +506,14 @@ static void invert_upper(const std::vector<double>& r, int b, double* inv, int l
   }
 }
 
-// v_out[i, col] = E_i u_col[i] / |E u_col|  (row-major [n, n_out]); one CTA per column
+// v_out[i, col] = E_i u_src[i] / |E u_src|  (row-major [n, n_out]), src = cols ? cols[col] : col;
+// one CTA per output column
 __global__ void k_mapback(const double* __restrict__ u, int64_t n, int n_out,
                           const double* __restrict__ left, const double* __restrict__ right,
-                          double* __restrict__ v_out) {
+                          const int* __restrict__ cols, double* __restrict__ v_out) {
   __shared__ double red[32];
   const int col = blockIdx.x;
-  const double* uc = u + (int64_t)col * n;
+  const double* uc = u + (int64_t)(cols ? cols[col] : col) * n;
   double ss = 0.0;
   for (int64_t i = threadIdx.x; i < n; i += blockDim.x) {
     const double e = sqrt((left ? left[i] : 1.0) / (right ? right[i] : 1.0));
@@ -652,11 +662,21 @@ typedef int (*sc_gather_fn)(void* user, int count);
 // basis vectors; a rank-deficient block goes one vector at a time instead.  T = V^T Op V is
 // banded (plus the arrow left by a thick restart); Ritz pairs come from T[0:P,0:P], their
 // residuals from the coupling rows T[P:P+b, 0:P].
+//
+// Locked set (windowed solve): `locked` holds n_locked orthonormal vectors of the symmetrised
+// space (vector-major, stride n) spanning eigenpairs found by earlier windows.  The start block,
+// every random direction and every product block are orthogonalised against it (classical
+// Gram-Schmidt, twice), so the solver finds the next n_values extremal pairs of Op restricted to
+// the complement; their Ritz vectors are appended at locked[n_locked..).  A residual counts as
+// converged when it is <= tol * max(|theta|max, scale): the complement's spectrum can sit far
+// below the operator's scale (a rank-deficient matrix leaves a cluster of rounding-level values),
+// and relative to the operator's scale is the accuracy its callers need.
 static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t row_begin,
                         int64_t n, int64_t lds, const double* delta, const double* left,
                         const double* right, double sign, int which, int64_t n_values,
                         int64_t n_vectors, double tol, int64_t max_matvecs, double* y_ext,
                         int slab, int64_t slab_len, sc_gather_fn gather, void* user,
+                        double* locked, int64_t n_locked, double scale,
                         double* w_host, double* v_dev, int64_t* stats_host, void* stream) {
   SC_REQUIRE(ctx && s && w_host && n > 0, "sc_eigh_extremal: bad arguments");
   SC_REQUIRE(n_values >= 1 && n_values <= 32 && n_vectors >= 0 && n_vectors <= n_values,
@@ -664,13 +684,14 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   SC_REQUIRE(n_vectors == 0 || v_dev, "sc_eigh_extremal: v_dev missing");
   SC_REQUIRE((reinterpret_cast<uintptr_t>(s) & 15) == 0 && lds % 4 == 0,
              "sc_eigh_extremal: S needs a 16-byte aligned base and lds %% 4 == 0");
+  SC_REQUIRE(n_locked >= 0 && (n_locked == 0 || locked), "sc_eigh_extremal: bad locked set");
   const int nev = (int)n_values;
   const int b = sc_eigh_block_size(n_values);
   const int m = 6 * b;                               // processed vectors before a thick restart
   const int jmax = m + b;                            // basis capacity
   const int keep_extra = std::max(8, nev / 2);
-  SC_REQUIRE(n >= 2 * (int64_t)jmax, "sc_eigh_extremal: n=%lld too small for the Lanczos basis "
-             "(%d); use sc_eigh_dense", (long long)n, jmax);
+  SC_REQUIRE(n - n_locked >= 2 * (int64_t)jmax, "sc_eigh_extremal: n=%lld (%lld locked) too small "
+             "for the Lanczos basis (%d); use sc_eigh_dense", (long long)n, (long long)n_locked, jmax);
   if (tol <= 0) tol = 1e-9;
   if (max_matvecs <= 0) max_matvecs = 20000;
   cudaStream_t st = as_stream(stream);
@@ -684,8 +705,14 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   SC_CUDA(small.alloc(sizeof(double) * (size_t)(2 * jmax + 8 + jmax * 64 + 2 * jmax * 16 + 256), st));
   const int bp_chunks = (int)((n + BP_CHUNK - 1) / BP_CHUNK);
   Scratch part;
-  SC_CUDA(part.alloc(sizeof(double) * (size_t)bp_chunks * jmax * 16, st));
+  const int proj_rows = n_locked > 0 ? std::max(jmax, LOCK_CHUNK) : jmax;
+  SC_CUDA(part.alloc(sizeof(double) * (size_t)bp_chunks * proj_rows * 16, st));
   double* partial = part.as<double>();
+  // locked-set coefficients: one chunk of the block form, or the whole set for one vector
+  Scratch lock_small;
+  if (n_locked > 0)
+    SC_CUDA(lock_small.alloc(sizeof(double) * (size_t)(LOCK_CHUNK * 16 + 2 * n_locked), st));
+  double* lh_dev = lock_small.as<double>();
   double* V = vb.as<double>();
   double* V2 = vb2.as<double>();
   double* tb = work.as<double>();                  // [b][ldtb] prescaled block
@@ -710,10 +737,30 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   double nrm2 = 0.0;
   uint64_t reseed = 1;
 
-  // V[at] <- a fresh random direction orthogonal to V[0..at)
+  // W (b vectors at stride n) <- W orthogonalised against the locked set: classical Gram-Schmidt
+  // twice, each sweep in chunks of LOCK_CHUNK locked vectors (the block kernels' coefficient
+  // tile); the coefficients are dropped, Op restricted to the complement is what is solved
+  auto deflate_block = [&](double* w) -> int {
+    for (int sweep = 0; sweep < 2; ++sweep)
+      for (int64_t j0 = 0; j0 < n_locked; j0 += LOCK_CHUNK) {
+        const int cnt = (int)std::min<int64_t>(LOCK_CHUNK, n_locked - j0);
+        const double* u = locked + (size_t)j0 * n;
+        SC_BLOCK_DISPATCH(b, {
+          if (int rc = launch_block_proj<B_>(u, n, cnt, w, partial, lh_dev, st)) return rc;
+          if (int rc = launch_block_axpy<B_>(u, n, cnt, lh_dev, w, st)) return rc;
+        });
+      }
+    return 0;
+  };
+
+  // V[at] <- a fresh random direction orthogonal to the locked set and to V[0..at)
   auto random_direction = [&](int at) -> int {
     double* w = wb;                                  // scratch: callers are done with wb[0]
     k_random_vec<<<gn, 256, 0, st>>>(w, n, 0x5CB200ull + 7919ull * reseed++); sc::launched();
+    if (n_locked > 0)
+      if (int rc = gram_schmidt2(locked, n, (int)n_locked, w, lh_dev, lh_dev + n_locked, nrm_dev,
+                                 nullptr, nullptr, &nrm2, st))
+        return rc;
     if (int rc = gram_schmidt2(V, n, at, w, h_dev, h2_dev, nrm_dev, nullptr, nullptr, &nrm2, st))
       return rc;
     k_scale_into<<<gn, 256, 0, st>>>(w, n, 1.0 / std::sqrt(nrm2), V + (size_t)at * n); sc::launched();
@@ -760,6 +807,7 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   {
     k_random_block<<<dim3(gn, b), 256, 0, st>>>(wb, n, 0x5CB200ull + 7919ull * reseed++); sc::launched();
     int status = -1;
+    if (int rc = deflate_block(wb)) return rc;
     if (int rc = gram_of(wb)) return rc;
     if (int rc = cholqr2(wb, tb, V, &status)) return rc;
     if (status != 0)
@@ -796,7 +844,7 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
       for (int q = 0; q < sz; ++q) Z[(size_t)q * sz + p] = zv[(size_t)q * sz + ord[p]];
     }
     mm = sz;
-    double tmax = 0.0;
+    double tmax = scale;
     for (int p = 0; p < sz; ++p) tmax = std::max(tmax, std::fabs(theta[p]));
     int ok = 0;
     for (int p = 0; p < nev && p < sz; ++p) {
@@ -828,6 +876,7 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
                                              right, sign, flip, n, wb); sc::launched();
     matvecs += b;
     ++passes;
+    if (int rc = deflate_block(wb)) return rc;
     // ---- block classical Gram-Schmidt (twice) of all b products against the basis, then
     // Cholesky-QR (twice) inside the block: T[0:J, P:P+b] = V^T W, T[J:J+b, P:P+b] = R
     SC_BLOCK_DISPATCH(b, {
@@ -838,6 +887,12 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
     });
     SC_CUDA(cudaMemcpyAsync(hb1.data(), hb1_dev, sizeof(double) * (size_t)J * b, cudaMemcpyDeviceToHost, st));
     SC_CUDA(cudaMemcpyAsync(hb2.data(), hb2_dev, sizeof(double) * (size_t)J * b, cudaMemcpyDeviceToHost, st));
+    // and against the locked set once more: what is left is small when the Krylov space nears an
+    // invariant subspace, and the locked components the first pass left at rounding level would
+    // grow by 1/|W| when it is normalised.  At the smallest end the locked directions are the
+    // extremal ones of the deflated operator (Op restricted to the complement is 0 on them), so
+    // any such growth is found.
+    if (int rc = deflate_block(wb)) return rc;
     if (int rc = gram_of(wb)) return rc;
     for (int p = 0; p < b; ++p)
       for (int q = 0; q < J; ++q) {
@@ -862,6 +917,10 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
       const int col = P + p;
       if (int rc = gram_schmidt2(V, n, J, w, h_dev, h2_dev, nrm_dev, hh.data(), hh2.data(), &nrm2, st))
         return rc;
+      if (n_locked > 0)                              // as above, before the division by beta
+        if (int rc = gram_schmidt2(locked, n, (int)n_locked, w, lh_dev, lh_dev + n_locked, nrm_dev,
+                                   nullptr, nullptr, &nrm2, st))
+          return rc;
       for (int q = 0; q < J; ++q) {
         const double v = hh[q] + hh2[q];
         Tat(q, col) += v;
@@ -922,6 +981,17 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
     }
   }
   for (int p = 0; p < nev; ++p) w_host[p] = flip * theta[p];
+  if (locked) {                                      // Ritz vectors of the window join the set
+    std::vector<double> zk((size_t)mm * 64, 0.0);
+    for (int q = 0; q < mm; ++q)
+      for (int p = 0; p < nev; ++p) zk[(size_t)q * 64 + p] = Z[(size_t)q * mm + p];
+    SC_CUDA(cudaMemcpyAsync(z_dev, zk.data(), sizeof(double) * (size_t)mm * 64,
+                            cudaMemcpyHostToDevice, st));
+    k_combine<<<dim3(gn, (unsigned)((nev + 7) / 8)), 256, 0, st>>>(V, n, mm, z_dev, 64, nev,
+                                                                  locked + (size_t)n_locked * n); sc::launched();
+    SC_LAUNCH_CHECK();
+    SC_CUDA(cudaStreamSynchronize(st));
+  }
   if (n_vectors > 0) {
     std::vector<double> zk((size_t)mm * 64, 0.0);
     for (int q = 0; q < mm; ++q)
@@ -930,7 +1000,7 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
                             cudaMemcpyHostToDevice, st));
     k_combine<<<dim3(gn, (unsigned)((n_vectors + 7) / 8)), 256, 0, st>>>(V, n, mm, z_dev, 64,
                                                                         (int)n_vectors, V2); sc::launched();
-    k_mapback<<<(unsigned)n_vectors, 512, 0, st>>>(V2, n, (int)n_vectors, left, right, v_dev); sc::launched();
+    k_mapback<<<(unsigned)n_vectors, 512, 0, st>>>(V2, n, (int)n_vectors, left, right, nullptr, v_dev); sc::launched();
     SC_LAUNCH_CHECK();
     SC_CUDA(cudaStreamSynchronize(st));
   }
@@ -970,8 +1040,34 @@ extern "C" int sc_eigh_extremal(sc_context* ctx, const float* s, int64_t n, int6
                                 double tol, int64_t max_matvecs, double* w_host, double* v_dev,
                                 int64_t* stats_host, void* stream) {
   return lanczos_impl(ctx, s, n, 0, n, lds, delta, left, right, sign, which, n_values, n_vectors,
-                      tol, max_matvecs, nullptr, 0, 0, nullptr, nullptr, w_host, v_dev, stats_host,
-                      stream);
+                      tol, max_matvecs, nullptr, 0, 0, nullptr, nullptr, nullptr, 0, 0.0, w_host,
+                      v_dev, stats_host, stream);
+}
+
+extern "C" int sc_eigh_extremal_locked(sc_context* ctx, const float* s, int64_t n, int64_t lds,
+                                       const double* delta, const double* left, const double* right,
+                                       double sign, int which, int64_t n_values, double tol,
+                                       int64_t max_matvecs, double scale, double* locked,
+                                       int64_t n_locked, double* w_host, int64_t* stats_host,
+                                       void* stream) {
+  SC_REQUIRE(locked, "sc_eigh_extremal_locked: locked buffer missing");
+  return lanczos_impl(ctx, s, n, 0, n, lds, delta, left, right, sign, which, n_values, 0, tol,
+                      max_matvecs, nullptr, 0, 0, nullptr, nullptr, locked, n_locked, scale, w_host,
+                      nullptr, stats_host, stream);
+}
+
+extern "C" int sc_eigh_mapback(sc_context* ctx, const double* u, int64_t n, const int* cols_host,
+                               int64_t k, const double* left, const double* right, double* v_out,
+                               void* stream) {
+  SC_REQUIRE(ctx && u && cols_host && v_out && n > 0 && k > 0, "sc_eigh_mapback: bad arguments");
+  cudaStream_t st = as_stream(stream);
+  Scratch cols;
+  SC_CUDA(cols.alloc(sizeof(int) * (size_t)k, st));
+  SC_CUDA(cudaMemcpyAsync(cols.as<int>(), cols_host, sizeof(int) * (size_t)k, cudaMemcpyHostToDevice, st));
+  k_mapback<<<(unsigned)k, 512, 0, st>>>(u, n, (int)k, left, right, cols.as<int>(), v_out); sc::launched();
+  SC_LAUNCH_CHECK();
+  SC_CUDA(cudaStreamSynchronize(st));             // cols_host may be released on return
+  return 0;
 }
 
 extern "C" int sc_eigh_extremal_sharded(sc_context* ctx, const float* s_block, int64_t rows,
@@ -989,7 +1085,7 @@ extern "C" int sc_eigh_extremal_sharded(sc_context* ctx, const float* s_block, i
              "sc_eigh_extremal_sharded: rank `slab` must own rows [slab*slab_len, +rows)");
   return lanczos_impl(ctx, s_block, rows, row_begin, n, lds, delta, left, right, sign, which,
                       n_values, n_vectors, tol, max_matvecs, y_slabs, slab, slab_len, gather, user,
-                      w_host, v_dev, stats_host, stream);
+                      nullptr, 0, 0.0, w_host, v_dev, stats_host, stream);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1069,7 +1165,7 @@ extern "C" int sc_krylov_combine(sc_context* ctx, const double* v, int64_t n, in
 extern "C" int sc_krylov_columns(sc_context* ctx, const double* u, int64_t n, int64_t k, double* v_out,
                                  void* stream) {
   SC_REQUIRE(ctx && u && v_out && n > 0 && k > 0, "sc_krylov_columns: bad arguments");
-  k_mapback<<<(unsigned)k, 512, 0, as_stream(stream)>>>(u, n, (int)k, nullptr, nullptr, v_out); sc::launched();
+  k_mapback<<<(unsigned)k, 512, 0, as_stream(stream)>>>(u, n, (int)k, nullptr, nullptr, nullptr, v_out); sc::launched();
   SC_LAUNCH_CHECK();
   return 0;
 }

@@ -141,6 +141,8 @@ class Engine:
       "sc_eigh_dense": "utils.compute_sorted_eigenvectors",
       "sc_eigh_extremal": "utils.compute_sorted_eigenvectors",
       "sc_eigh_extremal_sharded": "utils.compute_sorted_eigenvectors",
+      "sc_eigh_extremal_locked": "utils.compute_sorted_eigenvectors",
+      "sc_eigh_mapback": "utils.compute_sorted_eigenvectors",
       "sc_kmeans": "custom_distance_kmeans.run_kmeans", "sc_row_renorm": "spectral_clusterer.row_wise_renorm",
       "sc_affinity_stats": "fallback_clusterer.check_single_cluster",
       "sc_gmm_band_pass": "fallback_clusterer.check_single_cluster",
@@ -348,6 +350,31 @@ class Engine:
                 int(max_matvecs), wp, _ptr(v), stats.ctypes.data_as(ctypes.c_void_p),
                 self.stream)
     return w[:n_values], v[:, :n_vectors], stats
+
+  def eigh_window(self, s, n, delta, left, right, sign, which, n_values, locked, n_locked, scale,
+                  tol=1e-9, max_matvecs=0):
+    """The next n_values extremal eigenvalues (host fp64) on the complement of locked[:n_locked]
+    (device fp64 [capacity, n]); their symmetrised-space vectors land in locked[n_locked:]."""
+    w = np.empty(n_values, dtype=np.float64)
+    stats = np.zeros(4, dtype=np.int64)
+    assert locked.shape[0] >= n_locked + n_values and locked.shape[1] == n and locked.is_contiguous()
+    self.call("sc_eigh_extremal_locked", _ptr(s), n, s.stride(0), _ptr(delta), _ptr(left),
+              _ptr(right), float(sign), int(which), n_values, float(tol), int(max_matvecs),
+              float(scale), _ptr(locked), n_locked, w.ctypes.data_as(ctypes.c_void_p),
+              stats.ctypes.data_as(ctypes.c_void_p), self.stream)
+    return w, stats
+
+  def eigh_mapback(self, u, n, cols, left, right):
+    """Eigenvectors (device fp64 [n, len(cols)]) of the operator from the symmetrised-space
+    vectors u[cols] (device fp64 [*, n])."""
+    t = torch()
+    idx = np.ascontiguousarray(cols, dtype=np.int32)
+    v = t.empty((n, max(len(idx), 1)), dtype=t.float64, device=self.device)
+    if len(idx):
+      assert int(idx.min()) >= 0 and int(idx.max()) < u.shape[0] and u.is_contiguous()
+      self.call("sc_eigh_mapback", _ptr(u), n, idx.ctypes.data_as(ctypes.c_void_p), len(idx),
+                _ptr(left), _ptr(right), _ptr(v), self.stream)
+    return v[:, :len(idx)]
 
   def eigh_dense_pick(self, s, n, delta, left, right, sign, which, picker):
     """Full spectrum by the dense solver; `picker(w) -> count` (host) decides from the sorted

@@ -23,6 +23,7 @@ from . import autotune as autotune_lib
 from . import constraint as constraint_lib
 from . import custom_distance_kmeans
 from . import device as dev
+from . import eigen_windows
 from . import fallback_clusterer
 from . import laplacian as laplacian_lib
 from . import refinement
@@ -41,6 +42,9 @@ EigenGapType = utils.EigenGapType
 
 # The block Lanczos solver (sc_eigh_extremal) finds at most this many eigenpairs.
 LANCZOS_MAX_PAIRS = 32
+# The dense solver (sc_eigh_dense) takes n x n operators up to this n; above it, more pairs than
+# one Lanczos solve finds come from the windowed solve (eigen_windows.py).
+DENSE_MAX_N = 32768
 
 
 def lanczos_basis(limit: int) -> int:
@@ -146,18 +150,39 @@ class SpectralClusterer:
     n_vectors = min(n, max(limit, self.min_clusters or 0))
     op = (refined.s, n, delta, left, right, sign)
     counted = None          # (k, gap) when the solver already ran the eigengap
+    top = None              # lambda_max when w is a prefix of an ascending spectrum
     if not refined.symmetric:
       # not symmetric nor diagonally similar to a symmetric matrix (e.g. RowWiseThreshold without
       # Symmetrize): np.linalg.eig + .real semantics (utils.py:59-61) by Krylov-Schur
       from . import arnoldi
       solver = "krylov-schur"
-      w, v, stats = arnoldi.eig_extremal_device(eng, *op, not descend, limit, n_vectors)
-      top_solve = lambda: arnoldi.eig_extremal_device(eng, *op, False, 1, 0)[0]
+      if limit == n and n > arnoldi.FULL_SPECTRUM_LIMIT:
+        # max_clusters=None: only the prefix that settles the eigengap (eigen_windows.py)
+        w, v, stats, top = eigen_windows.grow_krylov_schur(
+            eng, op, descend, self.min_clusters, self.stop_eigenvalue, self.eigengap_type)
+        top_solve = None
+      else:
+        w, v, stats = arnoldi.eig_extremal_device(eng, *op, not descend, limit, n_vectors)
+        top_solve = lambda: arnoldi.eig_extremal_device(eng, *op, False, 1, 0)[0]
     elif n > eng.dense_eig_max and lanczos_fits(n, limit):
       solver = "lanczos"
       w, v, stats = eng.eigh(*op, which, limit, n_vectors, False)
       stats = stats.tolist()
       top_solve = lambda: eng.eigh(*op, nat.EIG_LARGEST, 1, 0, False)[0]
+    elif n > DENSE_MAX_N:
+      # more pairs than one Lanczos solve finds, above the dense solver's n: windows of block
+      # Lanczos on the complement of the pairs found, until the eigengap is decided
+      solver, top_solve = "lanczos-windows", None
+      ops = eigen_windows.DeviceOps(eng, *op, which, capacity=min(
+          n, eigen_windows.MAX_WINDOW_PAIRS,
+          max(limit, self.min_clusters or 0) + eigen_windows.WINDOW_PAIRS))
+      prefix = eigen_windows.solve(ops, descend, self.max_clusters, self.min_clusters,
+                                   self.stop_eigenvalue, self.eigengap_type, n=n)
+      w, top = prefix.values[:limit], prefix.lambda_max
+      counted = self._count_clusters(w, descend, top)
+      columns = min(len(w), max(counted[0], self.min_clusters or 0, 1))
+      v = ops.vectors(prefix.order[:columns])
+      stats = ops.stats
     else:
       # the dense solver (Householder tridiagonalisation, 4/3 n^3): small matrices, and
       # max_clusters=None / > 31 (every eigenvalue, or more pairs than Lanczos finds, is needed)
@@ -177,18 +202,19 @@ class SpectralClusterer:
         self.eigengap_type == EigenGapType.NormalizedDiff):
       # np.max(eigenvalues) of the full spectrum (utils.py:109): one more extremal solve
       w = np.concatenate([w, top_solve()])
-    k, gap = counted or self._count_clusters(w, descend)
+    k, gap = counted or self._count_clusters(w, descend, top)
     self.last_details = dict(eigenvalues=np.array(w[:limit]), n_clusters_raw=k, max_gap=gap,
                              solver=solver, lanczos_stats=stats)
     return w, v, k, gap
 
-  def _count_clusters(self, eigenvalues, descend: bool):
+  def _count_clusters(self, eigenvalues, descend: bool, max_eigenvalue=None):
     """utils.compute_number_of_clusters with this clusterer's options -> (k, max gap); only a
-    descending spectrum stops at stop_eigenvalue."""
+    descending spectrum stops at stop_eigenvalue.  `max_eigenvalue`: lambda_max of a spectrum of
+    which `eigenvalues` is an ascending prefix."""
     stop = dict(stop_eigenvalue=self.stop_eigenvalue) if descend else {}
     return utils.compute_number_of_clusters(eigenvalues, max_clusters=self.max_clusters,
                                             eigengap_type=self.eigengap_type, descend=descend,
-                                            **stop)
+                                            max_eigenvalue=max_eigenvalue, **stop)
 
   def _compute_eigenvectors_ncluster(self, affinity, constraint_matrix=None):
     """(eigenvectors, n_clusters, max eigengap) for an affinity matrix.

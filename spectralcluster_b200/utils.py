@@ -60,11 +60,15 @@ def compute_number_of_clusters(eigenvalues: np.ndarray,
                                stop_eigenvalue: float = 1e-2,
                                eigengap_type: EigenGapType = EigenGapType.Ratio,
                                descend: bool = True,
-                               eps: float = EPS) -> typing.Tuple[int, float]:
+                               eps: float = EPS,
+                               max_eigenvalue: typing.Optional[float] = None
+                               ) -> typing.Tuple[int, float]:
   """Maximum-eigengap estimate of the cluster count (host logic on <= max_clusters+1 values).
 
   Returns (number of clusters, the winning gap).  Descending spectra stop at the first
-  eigenvalue below `stop_eigenvalue`; ascending spectra skip the (zero) first eigenvalue."""
+  eigenvalue below `stop_eigenvalue`; ascending spectra skip the (zero) first eigenvalue.
+  `max_eigenvalue` stands in for np.max(eigenvalues) when `eigenvalues` is a prefix of the
+  spectrum that lacks its largest value (NormalizedDiff normalises by it)."""
   if not isinstance(eigengap_type, EigenGapType):
     raise TypeError("eigengap_type must be a EigenGapType")
   if eigengap_type not in (EigenGapType.Ratio, EigenGapType.NormalizedDiff):
@@ -76,7 +80,9 @@ def compute_number_of_clusters(eigenvalues: np.ndarray,
   use_ratio = eigengap_type == EigenGapType.Ratio
 
   def gap(big, small):
-    return big / (small + eps) if use_ratio else (big - small) / np.max(w)
+    if use_ratio:
+      return big / (small + eps)
+    return (big - small) / (np.max(w) if max_eigenvalue is None else max_eigenvalue)
 
   winner, widest = 0, 0
   if descend:
