@@ -28,6 +28,7 @@ struct KmState {
   int iters;
   int best_trial;
   int empty_cluster;
+  int nonfinite;      // bit 0: an embedding element is NaN, bit 1: one is +-inf
 };
 
 // ---- centring ---------------------------------------------------------------------------
@@ -41,18 +42,24 @@ __global__ void k_col_mean(const double* __restrict__ e, int64_t n, int64_t kd,
   if (threadIdx.x == 0) mean[f] = s / (double)n;
 }
 
+// Also flags non-finite input in st->nonfinite: scikit-learn's fit refuses it (check_array).
 __global__ void k_center(const double* __restrict__ e, int64_t n, int64_t kd,
                          const double* __restrict__ mean, double* __restrict__ x,
-                         double* __restrict__ xsq) {
+                         double* __restrict__ xsq, KmState* st) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   double ss = 0.0;
+  int bad = 0;
   for (int64_t f = 0; f < kd; ++f) {
-    const double v = e[i * kd + f] - mean[f];
+    const double ef = e[i * kd + f];
+    if (isnan(ef)) bad |= 1;
+    else if (isinf(ef)) bad |= 2;
+    const double v = ef - mean[f];
     x[i * kd + f] = v;
     ss += v * v;
   }
   xsq[i] = ss;
+  if (bad) atomicOr(&st->nonfinite, bad);
 }
 
 // ---- k-means++ ---------------------------------------------------------------------------
@@ -313,6 +320,7 @@ __global__ void k_state_init(KmState* st) {
   st->iters = 0;
   st->best_trial = 0;
   st->empty_cluster = 0;
+  st->nonfinite = 0;
 }
 
 __global__ void k_row_renorm(double* __restrict__ e, int64_t n, int64_t k) {
@@ -381,7 +389,7 @@ extern "C" int sc_kmeans(sc_context* ctx, const double* e, int64_t n, int64_t k_
                             cudaMemcpyHostToDevice, st));
   // ---- stage 1: scikit-learn seeding + one Lloyd iteration
   k_col_mean<<<(unsigned)k_dim, KT, 0, st>>>(e, n, k_dim, mean); sc::launched();
-  k_center<<<nb, KT, 0, st>>>(e, n, k_dim, mean, x, xsq); sc::launched();
+  k_center<<<nb, KT, 0, st>>>(e, n, k_dim, mean, x, xsq, state); sc::launched();
   k_kpp_first<<<nb, KT, 0, st>>>(x, xsq, n, k_dim, first_center, closest, part, centers); sc::launched();
   k_kpp_reduce_pot<<<1, KT, 0, st>>>(part, nb, state); sc::launched();
   SC_LAUNCH_CHECK();
@@ -416,6 +424,9 @@ extern "C" int sc_kmeans(sc_context* ctx, const double* e, int64_t n, int64_t k_
     SC_LAUNCH_CHECK();
     SC_CUDA(cudaMemcpyAsync(&hs, state, sizeof(hs), cudaMemcpyDeviceToHost, st));
     SC_CUDA(cudaStreamSynchronize(st));
+    // scikit-learn's wording (sklearn/utils/validation.py, _assert_all_finite): NaN first
+    SC_REQUIRE(!(hs.nonfinite & 1), "Input X contains NaN.");
+    SC_REQUIRE(!hs.nonfinite, "Input X contains infinity or a value too large for dtype('float64').");
     if (hs.done) break;
     SC_REQUIRE(launched <= max_iter + 8, "sc_kmeans: stop rule never fired (internal error)");
   }
