@@ -341,8 +341,26 @@ int sc_row_renorm(sc_context* ctx, double* e, int64_t n, int64_t k, void* stream
 /* e is fp64 [n,k_dim] on the device.  Seeding = scikit-learn KMeans(init="k-means++",
  * max_iter=1, random_state=0, n_init="auto") restated on the device: `first_center` and the
  * uniform draws u[(k-1)*trials] come from the caller's np.random.RandomState(0) (host RNG
- * logic only).  metric 0 = cosine, 1 = euclidean.  labels_host int64[n].  SYNCHRONOUS.
- * iters_host (may be NULL) receives the number of assignment passes. */
+ * logic only).  metric is one of the SC_KMEANS_* codes below: stage 2 uses that scipy cdist metric
+ * with scipy's special values (NaN, inf) and np.argmin's rule for the new codes (the first NaN
+ * wins, else the first minimum).  seuclidean's V and mahalanobis's VI = inv(cov)^T are recomputed
+ * every pass over the n + k stacked rows, as scipy's validators do; mahalanobis refuses
+ * n + k <= k_dim with scipy's ValueError wording and fails with "Singular matrix" (numpy's
+ * LinAlgError) on an exactly zero pivot.  minkowski with p = 2 is euclidean.  labels_host
+ * int64[n].  SYNCHRONOUS.  iters_host (may be NULL) receives the number of assignment passes. */
+enum {
+  SC_KMEANS_COSINE = 0,
+  SC_KMEANS_EUCLIDEAN = 1,
+  SC_KMEANS_SQEUCLIDEAN = 2,
+  SC_KMEANS_CITYBLOCK = 3,
+  SC_KMEANS_CHEBYSHEV = 4,
+  SC_KMEANS_CANBERRA = 5,
+  SC_KMEANS_BRAYCURTIS = 6,
+  SC_KMEANS_CORRELATION = 7,
+  SC_KMEANS_JENSENSHANNON = 8,
+  SC_KMEANS_SEUCLIDEAN = 9,
+  SC_KMEANS_MAHALANOBIS = 10
+};
 int sc_kmeans(sc_context* ctx, const double* e, int64_t n, int64_t k_dim, int64_t k,
               int64_t first_center, const double* u_host, int64_t trials, int metric,
               int64_t max_iter, double tol, int64_t* labels_host, int64_t* iters_host,

@@ -12,7 +12,27 @@ import numpy as np
 
 from . import device as dev
 
-_METRICS = {"cosine": 0, "euclidean": 1}
+# scipy.spatial.distance's numeric metrics and their spellings (scipy's _METRICS[name].aka) ->
+# sc_kmeans metric code (SC_KMEANS_* in include/spectralcluster_b200.h).  A name can only carry
+# minkowski's default p = 2, which scipy evaluates as euclidean.
+_ALIASES = {
+    "cosine": {"cosine", "cos"},
+    "euclidean": {"euclidean", "euclid", "eu", "e"},
+    "sqeuclidean": {"sqeuclidean", "sqeuclid", "sqe"},
+    "cityblock": {"cityblock", "cblock", "cb", "c"},
+    "chebyshev": {"chebyshev", "chebychev", "cheby", "cheb", "ch"},
+    "minkowski": {"minkowski", "mi", "m", "pnorm"},
+    "canberra": {"canberra"},
+    "braycurtis": {"braycurtis"},
+    "correlation": {"correlation", "co"},
+    "jensenshannon": {"jensenshannon", "js"},
+    "seuclidean": {"seuclidean", "se", "s"},
+    "mahalanobis": {"mahalanobis", "mahal", "mah"},
+}
+_CODES = {"cosine": 0, "euclidean": 1, "sqeuclidean": 2, "cityblock": 3, "chebyshev": 4,
+          "minkowski": 1, "canberra": 5, "braycurtis": 6, "correlation": 7, "jensenshannon": 8,
+          "seuclidean": 9, "mahalanobis": 10}
+_METRICS = {alias: _CODES[name] for name, akas in _ALIASES.items() for alias in akas}
 
 
 def run_kmeans(spectral_embeddings, n_clusters: int,
@@ -20,10 +40,13 @@ def run_kmeans(spectral_embeddings, n_clusters: int,
   """Cluster the rows of `spectral_embeddings` (host ndarray or device fp64 tensor) into
   `n_clusters` groups; returns int64 labels on the host.
 
-  "cosine" (every BASELINE configuration) and "euclidean" run entirely on the device.  The other
-  forms the reference accepts -- any scipy.spatial.distance metric name or callable
-  (custom_distance_kmeans.py:37-47; None fails in the reference, and here) -- are host code on the [n, k]
-  embeddings (k <= a few dozen columns; the N x N work is long done), exactly like the reference."""
+  Every numeric scipy.spatial.distance metric name (cosine, euclidean, sqeuclidean, cityblock,
+  chebyshev, minkowski, canberra, braycurtis, correlation, jensenshannon, seuclidean, mahalanobis,
+  and scipy's other spellings of them) runs entirely on the device, with scipy's special values.
+  A singular mahalanobis covariance raises numpy.linalg.LinAlgError, as np.linalg.inv does.  The
+  other forms the reference accepts -- callables, hamming and the boolean metrics (degenerate on
+  real-valued embeddings; custom_distance_kmeans.py:37-47; None fails in the reference, and
+  here) -- are host code on the [n, k] embeddings, exactly like the reference."""
   eng = dev.Engine.get()          # no CUDA device -> RuntimeError, whatever the metric
   if isinstance(custom_dist, str) and custom_dist in _METRICS:
     t = dev.torch()
@@ -50,7 +73,8 @@ def run_kmeans(spectral_embeddings, n_clusters: int,
 @dataclasses.dataclass
 class CustomKMeans:
   """Lloyd iterations under an arbitrary scipy distance (custom_distance_kmeans.py:55-141), host
-  arrays; `run_kmeans` uses the CUDA implementation of the same loop for cosine / euclidean."""
+  arrays; `run_kmeans` uses the CUDA implementation of the same loop for every numeric metric
+  name."""
   n_clusters: typing.Optional[int] = None
   centroids: typing.Optional[np.ndarray] = None
   max_iter: int = 10

@@ -410,7 +410,9 @@ class Engine:
     self.call("sc_row_renorm", _ptr(e), int(e.shape[0]), int(e.shape[1]), self.stream)
 
   def kmeans(self, e, k, metric, max_iter, tol=0.001):
-    """run_kmeans on a contiguous device fp64 [n, k_dim] array -> host int64 labels."""
+    """run_kmeans on a contiguous device fp64 [n, k_dim] array -> (host int64 labels, passes).
+    `metric` is an SC_KMEANS_* code.  Errors are ValueError, except a singular mahalanobis
+    covariance: numpy.linalg.LinAlgError("Singular matrix"), as np.linalg.inv raises it."""
     n, kd = int(e.shape[0]), int(e.shape[1])
     # scikit-learn's draws: RandomState(0).choice(n, p=uniform) then uniform(size=trials) per
     # additional centre (sklearn/cluster/_kmeans.py:231, :249).  Host RNG logic only.
@@ -421,10 +423,15 @@ class Engine:
         [rs.uniform(size=trials) for _ in range(k - 1)], dtype=np.float64).reshape(-1)
     labels = np.empty(n, dtype=np.int64)
     iters = np.zeros(1, dtype=np.int64)
-    self.call("sc_kmeans", _ptr(e), n, kd, int(k), first,
-              u.ctypes.data_as(ctypes.c_void_p) if u.size else None, trials, int(metric),
-              int(max_iter), float(tol), labels.ctypes.data_as(ctypes.c_void_p),
-              iters.ctypes.data_as(ctypes.c_void_p), self.stream, exc=ValueError)
+    try:
+      self.call("sc_kmeans", _ptr(e), n, kd, int(k), first,
+                u.ctypes.data_as(ctypes.c_void_p) if u.size else None, trials, int(metric),
+                int(max_iter), float(tol), labels.ctypes.data_as(ctypes.c_void_p),
+                iters.ctypes.data_as(ctypes.c_void_p), self.stream, exc=ValueError)
+    except ValueError as err:
+      if str(err) == "Singular matrix":
+        raise np.linalg.LinAlgError("Singular matrix") from None
+      raise
     return labels, int(iters[0])
 
   def cosine_distances(self, x_dev):
