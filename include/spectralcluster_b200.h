@@ -148,7 +148,8 @@ int sc_split_planes(sc_context* ctx, const float* a, int64_t n, int64_t lda, voi
  * neither (tensor-core engine only), receive max_j s[i,j] and sum_j s[i,j] from the GEMM epilogue: the
  * reductions of the following RowWiseNormalize (refinement.py:243) and of the Laplacian degree
  * (laplacian.py:41) without another pass over S.  The fused maximum assumes max_j s[i,j] >= 0,
- * which holds for every y (s[i,i] = |y_i|^2). */
+ * which holds for every y (s[i,i] = |y_i|^2).  s == NULL (tensor-core engine, rowmax given) is the
+ * statistics-only form: the same GEMM and epilogue reductions, bit for bit, with no store of S. */
 int sc_diffuse(sc_context* ctx, int engine, int precision, const float* y, int64_t ldy,
                const void* hi, const void* lo, int64_t ldh, int64_t n, float* s, int64_t lds,
                float* rowmax, double* rowsum, void* stream);
@@ -179,6 +180,35 @@ int sc_affinity_cosine_block(sc_context* ctx, int precision, const void* hi, con
                              int64_t ldh, int64_t n, int64_t d, int64_t row_begin,
                              int64_t row_count, float* a_block, int64_t lda,
                              float* rowmax_offdiag_block, void* stream);
+/* ---- row panels of the single-GPU factored route (no N x N fp32 matrix is ever allocated).
+ * sc_affinity_cosine_panel: rows [row_begin, row_begin+row_count) of the sc_affinity_cosine
+ * matrix (tensor-core engine), equal to them bit for bit -- row_begin % 128 == 0, so the panel's
+ * tiles are the whole-matrix tiles, those below the diagonal stored as the transpose of their
+ * mirror tile as the symmetric launch stores them.  crop_panel (may be NULL) receives the
+ * CropDiagonal values of those rows, indexed from row_begin.
+ * sc_blur_upper_rowmax_block: pass 1 of the symmetric blur pair (sc_blur_upper_rowmax) for the
+ * output rows [row_begin, row_end) (row_begin % 32 == 0) of a panel `a` holding global rows
+ * [in_row_base, in_row_base+in_rows), halo included; b_out holds rows [row_begin, row_end) of the
+ * upper tiles of blur(a).  Their row and column maxima are folded into rowmax_accum (global
+ * length n), which is NOT reset: zero it once, then run every panel.
+ * sc_threshold_symmetrize_upper_block: pass 2 (sc_threshold_symmetrize_upper) for the 64 x 64
+ * tile pairs (TI, TJ >= TI) whose rows TI lie in [row_begin, row_end) (row_begin % 64 == 0,
+ * row_end % 64 == 0 or row_end == n), from such a b panel; y / hi / lo are the full-size outputs
+ * and receive Y(i,j) and its mirror Y(j,i). */
+int sc_affinity_cosine_panel(sc_context* ctx, int precision, const void* hi, const void* lo,
+                             int64_t ldh, int64_t n, int64_t d, int64_t row_begin,
+                             int64_t row_count, float* a_panel, int64_t lda, float* crop_panel,
+                             void* stream);
+int sc_blur_upper_rowmax_block(sc_context* ctx, const float* a, int64_t n, int64_t lda,
+                               int64_t in_row_base, int64_t in_rows, int64_t row_begin,
+                               int64_t row_end, const float* diag_override, double sigma,
+                               int zero_diagonal, float* b_out, int64_t ldb, float* rowmax_accum,
+                               void* stream);
+int sc_threshold_symmetrize_upper_block(sc_context* ctx, const float* b, int64_t n, int64_t ldb,
+                                        int64_t row_begin, int64_t row_end, const float* rowmax,
+                                        double p, double mult, int binarize,
+                                        int preserve_diagonal, int sym_type, float* y, int64_t ldy,
+                                        void* hi, void* lo, int64_t ldh, void* stream);
 /* Blur statistics / blur+threshold+symmetrize for global rows [row_begin, row_end) when `a` holds
  * global rows [in_row_base, in_row_base+in_rows) (owned rows + the blur halo, recomputed locally
  * rather than exchanged).  Output buffers start at global row row_begin; diag_override, rowmax and
@@ -310,6 +340,23 @@ int sc_eigh_extremal_sharded(sc_context* ctx, const float* s_block, int64_t rows
  * exported so that the kernel has its own parity test against a float64 product. */
 int sc_block_product(sc_context* ctx, const float* s, int64_t rows, int64_t n, int64_t lds,
                      const double* t, int64_t ldt, int b, double* y, int64_t ldy, void* stream);
+
+/* sc_block_product with an fp16 matrix `s` (16-byte aligned, lds % 8 == 0), converted exactly to
+ * fp64 for the products: the block product of the factored operator below. */
+int sc_block_product_f16(sc_context* ctx, const void* s, int64_t rows, int64_t n, int64_t lds,
+                         const double* t, int64_t ldt, int b, double* y, int64_t ldy, void* stream);
+
+/* sc_eigh_extremal on the factored operator S = Y Y^T, where y_hi is the fp16 hi plane of a
+ * bitwise-symmetric Y (n x n, leading dimension ldy % 8 == 0) and S is never formed: each block
+ * product is Y (Y T) by two sc_block_product_f16 passes through an [b][n] fp64 intermediate (2 + 2
+ * B per element, the bytes of one pass over an fp32 S).  fp16 -> fp64 is exact, so this is the
+ * exact product of Y up to the fp64 accumulation; a stored S is its fp32-accumulated rounding.
+ * Arguments and results otherwise as sc_eigh_extremal.  SYNCHRONOUS. */
+int sc_eigh_extremal_factored(sc_context* ctx, const void* y_hi, int64_t n, int64_t ldy,
+                              const double* delta, const double* left, const double* right,
+                              double sign, int which, int64_t n_values, int64_t n_vectors,
+                              double tol, int64_t max_matvecs, double* w_host, double* v_dev,
+                              int64_t* stats_host, void* stream);
 
 /* ---- Krylov primitives of the general (non-symmetrisable) eigen path: utils.py:59-61 is
  * np.linalg.eig + .real; sequences such as [RowWiseThreshold] alone leave a genuinely

@@ -87,6 +87,17 @@ PROTOTYPES = {
                                  c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_block_product": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, ctypes.c_int, c_ptr, c_i64,
                          c_ptr],
+    "sc_block_product_f16": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, ctypes.c_int, c_ptr,
+                             c_i64, c_ptr],
+    "sc_eigh_extremal_factored": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_dbl, c_int,
+                                  c_i64, c_i64, c_dbl, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_affinity_cosine_panel": [c_ptr, c_int, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64,
+                                 c_ptr, c_i64, c_ptr, c_ptr],
+    "sc_blur_upper_rowmax_block": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr,
+                                   c_dbl, c_int, c_ptr, c_i64, c_ptr, c_ptr],
+    "sc_threshold_symmetrize_upper_block": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_dbl,
+                                            c_dbl, c_int, c_int, c_int, c_ptr, c_i64, c_ptr, c_ptr,
+                                            c_i64, c_ptr],
     "sc_krylov_matvec": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     "sc_krylov_orthogonalize": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_krylov_scale": [c_ptr, c_ptr, c_i64, c_dbl, c_ptr, c_ptr],

@@ -1,6 +1,7 @@
 // Context, error reporting and the GEMM-backed entry points of the C ABI.
 #include "common.cuh"
 
+#include <algorithm>
 #include <atomic>
 #include <cstdlib>
 #include <cstring>
@@ -30,6 +31,9 @@ int gemm_nt_wgmma(const sc_context* ctx, int epi, int precision, const __half* a
                   int64_t ldb, int64_t M, int64_t N, int64_t K, float* C, int64_t ldc,
                   float* rowmax_offdiag, bool symmetric, int diag_shift, float* stat_rowmax,
                   double* stat_rowsum, float* mirror, int64_t ldm, cudaStream_t st);
+// rowops.cu
+int crop_diagonal_rows(const float* a, int64_t n, int64_t lda, int64_t row_begin, int64_t rows,
+                       float* diag_out, cudaStream_t st);
 
 }  // namespace sc
 
@@ -114,8 +118,9 @@ extern "C" int sc_affinity_cosine(sc_context* ctx, int engine, int precision, co
 extern "C" int sc_diffuse(sc_context* ctx, int engine, int precision, const float* y,
                           int64_t ldy, const void* hi, const void* lo, int64_t ldh, int64_t n,
                           float* s, int64_t lds, float* rowmax, double* rowsum, void* stream) {
-  SC_REQUIRE(ctx && s && n > 0, "sc_diffuse: bad arguments");
+  SC_REQUIRE(ctx && (s || rowmax) && n > 0, "sc_diffuse: bad arguments");
   SC_REQUIRE((rowmax == nullptr) == (rowsum == nullptr), "sc_diffuse: rowmax/rowsum come together");
+  SC_REQUIRE(s || engine == SC_GEMM_TCGEN05, "sc_diffuse: s == NULL needs the tensor-core engine");
   if (engine == SC_GEMM_SIMT_F64ACC) {
     SC_REQUIRE(y, "sc_diffuse: the SIMT engine needs the fp32 operand");
     SC_REQUIRE(!rowmax, "sc_diffuse: the SIMT engine has no fused row statistics");
@@ -148,6 +153,40 @@ extern "C" int sc_affinity_cosine_block(sc_context* ctx, int precision, const vo
                          ldh, h, l, ldh, row_count, n, d, a_block, lda, rowmax_offdiag_block,
                          /*symmetric=*/false, /*diag_shift=*/(int)row_begin, nullptr, nullptr,
                          nullptr, 0, as_stream(stream));
+}
+
+// Rows [row_begin, row_begin + row_count) of the sc_affinity_cosine matrix, bit for bit: one
+// 128-row strip at a time, the tiles on and above the diagonal computed directly and those below it
+// as the transpose of their mirror tile, as the symmetric whole-matrix launch does.
+extern "C" int sc_affinity_cosine_panel(sc_context* ctx, int precision, const void* hi,
+                                        const void* lo, int64_t ldh, int64_t n, int64_t d,
+                                        int64_t row_begin, int64_t row_count, float* a_panel,
+                                        int64_t lda, float* crop_panel, void* stream) {
+  SC_REQUIRE(ctx && hi && a_panel && n > 0 && d > 0 && row_begin >= 0 && row_count > 0 &&
+             row_begin + row_count <= n, "sc_affinity_cosine_panel: bad arguments");
+  SC_REQUIRE(row_begin % 128 == 0, "sc_affinity_cosine_panel: row_begin must be a multiple of 128");
+  SC_REQUIRE(lo || precision == SC_GEMM_SINGLE, "sc_affinity_cosine_panel: lo plane missing");
+  const __half* h = (const __half*)hi;
+  const __half* l = (const __half*)lo;
+  cudaStream_t st = as_stream(stream);
+  for (int64_t s0 = row_begin; s0 < row_begin + row_count; s0 += 128) {
+    const int64_t rows = std::min<int64_t>(128, row_begin + row_count - s0);   // rows of the panel
+    float* strip = a_panel + (s0 - row_begin) * lda;
+    // columns [s0, n): the diagonal tile and the tiles right of it
+    if (int rc = gemm_nt_wgmma(ctx, 1, precision, h + s0 * ldh, l ? l + s0 * ldh : nullptr, ldh,
+                               h + s0 * ldh, l ? l + s0 * ldh : nullptr, ldh, rows, n - s0, d,
+                               strip + s0, lda, nullptr, /*symmetric=*/false, 0, nullptr, nullptr,
+                               nullptr, 0, st))
+      return rc;
+    // columns [0, s0): tiles (rows of X[0, s0)) x (this strip), stored transposed only
+    if (s0 > 0)
+      if (int rc = gemm_nt_wgmma(ctx, 1, precision, h, l, ldh, h + s0 * ldh,
+                                 l ? l + s0 * ldh : nullptr, ldh, s0, rows, d, nullptr, 0, nullptr,
+                                 /*symmetric=*/false, 0, nullptr, nullptr, strip, lda, st))
+        return rc;
+  }
+  if (crop_panel) return crop_diagonal_rows(a_panel, n, lda, row_begin, row_count, crop_panel, st);
+  return 0;
 }
 
 extern "C" int sc_gemm_nt_planes(sc_context* ctx, int precision, const void* a_hi,

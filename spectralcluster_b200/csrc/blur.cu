@@ -586,8 +586,9 @@ __global__ void k_noblur(const BlurArgs g) {
 constexpr int UT = 64;
 
 struct UpperArgs {
-  const float* b;
-  int64_t n, ldb;
+  const float* b;            // rows [b_row0, ...) of the upper tiles of B
+  int64_t n, ldb, b_row0;
+  int64_t pair0;             // linear index of the first tile pair (a row panel starts past 0)
   int tiles;                 // ceil(n / UT)
   RuleArgs r;
 };
@@ -601,7 +602,7 @@ k_thrsym_upper(const UpperArgs g) {
   __shared__ float tile[UT][UT + 1];
   const RuleArgs& r = g.r;
   // linear index -> (TI, TJ) with TI <= TJ: row TI of the triangle starts at TI*T - TI(TI-1)/2
-  const int64_t T = g.tiles, idx = blockIdx.x;
+  const int64_t T = g.tiles, idx = g.pair0 + blockIdx.x;
   int64_t ti = (int64_t)(((2.0 * T + 1.0) - sqrt((2.0 * T + 1.0) * (2.0 * T + 1.0) - 8.0 * (double)idx)) * 0.5);
   while (ti > 0 && ti * T - ti * (ti - 1) / 2 > idx) --ti;
   while ((ti + 1) * T - (ti + 1) * ti / 2 <= idx) ++ti;
@@ -629,18 +630,18 @@ k_thrsym_upper(const UpperArgs g) {
     if (i < g.n) {
       float bv[4] = {0.0f, 0.0f, 0.0f, 0.0f};
       if (full4) {
-        const float4 v = ld_stream4(g.b + i * g.ldb + j);
+        const float4 v = ld_stream4(g.b + (i - g.b_row0) * g.ldb + j);
         bv[0] = v.x; bv[1] = v.y; bv[2] = v.z; bv[3] = v.w;
       } else {
 #pragma unroll
-        for (int t = 0; t < 4; ++t) bv[t] = (j + t < g.n) ? g.b[i * g.ldb + j + t] : 0.0f;
+        for (int t = 0; t < 4; ++t) bv[t] = (j + t < g.n) ? g.b[(i - g.b_row0) * g.ldb + j + t] : 0.0f;
       }
       if (diag_tile) {
         // below the diagonal, the mirror of the upper element: the computed blur is not bitwise
         // symmetric, and Y(i, j) must equal Y(j, i) = rule(b[j, i], m_j, m_i) exactly
 #pragma unroll
         for (int t = 0; t < 4; ++t)
-          if (j + t < i) bv[t] = g.b[(j + t) * g.ldb + i];
+          if (j + t < i) bv[t] = g.b[(j + t - g.b_row0) * g.ldb + i];
       }
       const float cut_i = r.m[i] * r.p;
       const int64_t dcol = diag_tile ? i - j : -1;             // column of (i, i) in the run
@@ -890,23 +891,74 @@ extern "C" int sc_blur_upper_rowmax(sc_context* ctx, const float* a, int64_t n, 
   return launch_band<EPI_UPPER>(g, bw, as_stream(stream));
 }
 
+// Pass 2 over the tile pairs (TI, TJ), TI <= TJ, whose rows TI lie in [row_begin, row_end); `b`
+// holds rows [row_begin, row_end) of the upper tiles of B.
+static int thrsym_upper_rows(const char* who, sc_context* ctx, const float* b, int64_t n,
+                             int64_t ldb, int64_t row_begin, int64_t row_end, const float* rowmax,
+                             double p, double mult, int binarize, int preserve_diagonal,
+                             int sym_type, float* y, int64_t ldy, void* hi, void* lo, int64_t ldh,
+                             void* stream) {
+  SC_REQUIRE(ctx && b && rowmax && n > 0, "%s: bad arguments", who);
+  SC_REQUIRE(0 <= row_begin && row_begin < row_end && row_end <= n && row_begin % UT == 0 &&
+             (row_end % UT == 0 || row_end == n),
+             "%s: the row range must start on a multiple of %d and end on one or at n", who, UT);
+  UpperArgs g = {};
+  if (int rc = rule_args(who, rowmax, p, mult, binarize, preserve_diagonal, sym_type, y, ldy, hi,
+                         lo, ldh, g.r))
+    return rc;
+  SC_REQUIRE(vec_ok_f32(b, ldb), "%s: `b` alignment", who);
+  g.b = b; g.n = n; g.ldb = ldb; g.b_row0 = row_begin;
+  g.tiles = (int)((n + UT - 1) / UT);
+  const int64_t T = g.tiles, t0 = row_begin / UT, t1 = (row_end + UT - 1) / UT;
+  g.pair0 = t0 * T - t0 * (t0 - 1) / 2;                     // first pair of tile row t0
+  const int64_t pairs = t1 * T - t1 * (t1 - 1) / 2 - g.pair0;
+  SC_REQUIRE(T * (T + 1) / 2 < (1LL << 31), "%s: n too large for the tile grid", who);
+  k_thrsym_upper<<<(unsigned)pairs, 256, 0, as_stream(stream)>>>(g); sc::launched();
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
 // Pass 2: y / planes <- sym(thr(b, m_i), thr(b, m_j)) for the WHOLE matrix from the upper tiles of b.
 extern "C" int sc_threshold_symmetrize_upper(sc_context* ctx, const float* b, int64_t n, int64_t ldb,
                                              const float* rowmax, double p, double mult,
                                              int binarize, int preserve_diagonal, int sym_type,
                                              float* y, int64_t ldy, void* hi, void* lo, int64_t ldh,
                                              void* stream) {
-  SC_REQUIRE(ctx && b && rowmax && n > 0, "sc_threshold_symmetrize_upper: bad arguments");
-  UpperArgs g = {};
-  if (int rc = rule_args("sc_threshold_symmetrize_upper", rowmax, p, mult, binarize,
-                         preserve_diagonal, sym_type, y, ldy, hi, lo, ldh, g.r))
-    return rc;
-  SC_REQUIRE(vec_ok_f32(b, ldb), "sc_threshold_symmetrize_upper: `b` alignment");
-  g.b = b; g.n = n; g.ldb = ldb;
-  g.tiles = (int)((n + UT - 1) / UT);
-  const int64_t pairs = (int64_t)g.tiles * (g.tiles + 1) / 2;
-  SC_REQUIRE(pairs < (1LL << 31), "sc_threshold_symmetrize_upper: n too large for the tile grid");
-  k_thrsym_upper<<<(unsigned)pairs, 256, 0, as_stream(stream)>>>(g); sc::launched();
-  SC_LAUNCH_CHECK();
-  return 0;
+  return thrsym_upper_rows("sc_threshold_symmetrize_upper", ctx, b, n, ldb, 0, n, rowmax, p, mult,
+                           binarize, preserve_diagonal, sym_type, y, ldy, hi, lo, ldh, stream);
+}
+
+// ---- row panels of the symmetric pair (one GPU, no N x N fp32 matrix).  Pass 1 over the rows
+// [row_begin, row_end) of a panel `a` that holds global rows [in_row_base, in_row_base + in_rows):
+// b_out (rows [row_begin, row_end)) <- the upper tiles of blur(a), and their row and column maxima
+// are folded into rowmax_accum, which the caller zero-fills once for all panels.
+extern "C" int sc_blur_upper_rowmax_block(sc_context* ctx, const float* a, int64_t n, int64_t lda,
+                                          int64_t in_row_base, int64_t in_rows, int64_t row_begin,
+                                          int64_t row_end, const float* diag_override,
+                                          double sigma, int zero_diagonal, float* b_out,
+                                          int64_t ldb, float* rowmax_accum, void* stream) {
+  SC_REQUIRE(ctx && a && b_out && rowmax_accum && n > 0, "sc_blur_upper_rowmax_block: bad arguments");
+  SC_REQUIRE(blur_radius(sigma) == 4,
+             "sc_blur_upper_rowmax_block: the symmetric pass is built for radius 4 (sigma ~ 1)");
+  SC_REQUIRE(row_begin % TTH == 0, "sc_blur_upper_rowmax_block: row_begin must be a multiple of %d", TTH);
+  SC_REQUIRE(vec_ok_f32(b_out, ldb), "blur: `out` needs a 16-byte aligned base and ldo %% 4 == 0");
+  if (int rc = check_block(n, in_row_base, in_rows, row_begin, row_end, sigma)) return rc;
+  SC_REQUIRE(row_end - row_begin <= 65535LL * 32, "sc_blur_upper_rowmax_block: too many rows");
+  BlurArgs g = blur_args(a, n, lda, in_row_base, row_begin, row_end, diag_override);
+  g.out = b_out; g.ldo = ldb; g.rowmax_out = rowmax_accum; g.stats_zero_diag = zero_diagonal;
+  BlurWeights bw;
+  make_weights(sigma, bw, g.radius);
+  return launch_band<EPI_UPPER>(g, bw, as_stream(stream));
+}
+
+// Pass 2 of a panel: the tile pairs whose first tile row lies in [row_begin, row_end), from the
+// panel's upper tiles of B (rows [row_begin, row_end), as pass 1 wrote them); Y and its mirror go
+// to the full-size outputs.
+extern "C" int sc_threshold_symmetrize_upper_block(
+    sc_context* ctx, const float* b, int64_t n, int64_t ldb, int64_t row_begin, int64_t row_end,
+    const float* rowmax, double p, double mult, int binarize, int preserve_diagonal, int sym_type,
+    float* y, int64_t ldy, void* hi, void* lo, int64_t ldh, void* stream) {
+  return thrsym_upper_rows("sc_threshold_symmetrize_upper_block", ctx, b, n, ldb, row_begin,
+                           row_end, rowmax, p, mult, binarize, preserve_diagonal, sym_type, y, ldy,
+                           hi, lo, ldh, stream);
 }

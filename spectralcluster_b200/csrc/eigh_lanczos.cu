@@ -91,14 +91,25 @@ constexpr int SYMM_ROWS = 256, SYMM_COLS = 32, SYMM_SP = 36, SYMM_TP = 36, SYMM_
 constexpr int SYMM_S_FLOATS = SYMM_ROWS * SYMM_SP;                       // 9,216 floats = 36,864 B
 constexpr int SYMM_STAGE_BYTES = SYMM_S_FLOATS * 4 + SYMM_MAXB * SYMM_TP * 8;   // + 4,608 B
 constexpr int SYMM_STAGES = 2;     // x 41,472 B: two CTAs (16 warps) per SM
+// The factored operator (sc_eigh_extremal_factored) stages an fp16 matrix in the same stage
+// buffers: 256 rows x 32 columns of fp16 at a row pitch of 40 halves (80 B: 16-byte aligned rows,
+// and the eight rows of an A fragment land on distinct bank quads).  fp16 -> fp64 is exact.
+template <typename T> struct SymmElem;
+template <> struct SymmElem<float> { static constexpr int SP = SYMM_SP; };
+template <> struct SymmElem<__half> { static constexpr int SP = 40; };
+static_assert(SYMM_ROWS * 40 * 2 <= SYMM_S_FLOATS * 4, "fp16 tile fits the fp32 stage");
+
+__device__ __forceinline__ double to_f64(float x) { return (double)x; }
+__device__ __forceinline__ double to_f64(__half x) { return (double)__half2float(x); }
 
 __device__ __forceinline__ void cp_async16_zfill(void* dst, const void* src, int src_bytes) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;"
                ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src), "r"(src_bytes) : "memory");
 }
 
+template <typename T>
 __global__ void __launch_bounds__(256, 2)
-k_symm_dmma(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
+k_symm_dmma(const T* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
             const double* __restrict__ t /*[b][ldt]*/, int64_t ldt, int b, int row_blocks,
             int64_t cols_per_split, double* __restrict__ partial /*[split][b][rows_pad]*/,
             int64_t rows_pad) {
@@ -109,23 +120,26 @@ k_symm_dmma(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
   const int64_t c_begin = (int64_t)split * cols_per_split;
   const int64_t c_end = min(n, c_begin + cols_per_split);
   const int chunks = (int)((c_end - c_begin + SYMM_COLS - 1) / SYMM_COLS);
-  auto stage_s = [&](int st) { return reinterpret_cast<float*>(symm_smem + (size_t)st * SYMM_STAGE_BYTES); };
+  constexpr int SP = SymmElem<T>::SP, GR = 16 / (int)sizeof(T);   // elements per 16-byte granule
+  auto stage_s = [&](int st) { return reinterpret_cast<T*>(symm_smem + (size_t)st * SYMM_STAGE_BYTES); };
   auto stage_t = [&](int st) {
     return reinterpret_cast<double*>(symm_smem + (size_t)st * SYMM_STAGE_BYTES + SYMM_S_FLOATS * 4);
   };
-  // fill: 256 rows x 8 16-byte granules of S (8 per thread), b rows x 16 granules of T
+  // fill: 256 rows x 8 (fp16: 4) 16-byte granules of S, 8 (4) per thread; b rows x 16 granules of T
   auto fill = [&](int ch, int st) {
     const int64_t c0 = c_begin + (int64_t)ch * SYMM_COLS;
-    float* ss = stage_s(st);
+    T* ss = stage_s(st);
+    constexpr int GPR = SYMM_COLS / GR;                // granules per row
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const int idx = threadIdx.x + k * 256;           // 0 .. 2047
-      const int r = idx >> 3, q = idx & 7;
+    for (int k = 0; k < SYMM_ROWS * GPR / 256; ++k) {
+      const int idx = threadIdx.x + k * 256;
+      const int r = idx / GPR, q = idx % GPR;
       const int64_t gr = (row0 + r < rows) ? row0 + r : rows - 1;
-      const int64_t gc = c0 + 4 * q;
+      const int64_t gc = c0 + GR * q;
       int64_t valid = c_end - gc;
-      valid = valid < 0 ? 0 : (valid > 4 ? 4 : valid);
-      cp_async16_zfill(ss + r * SYMM_SP + 4 * q, s + gr * lds + (valid > 0 ? gc : 0), (int)valid * 4);
+      valid = valid < 0 ? 0 : (valid > GR ? GR : valid);
+      cp_async16_zfill(ss + r * SP + GR * q, s + gr * lds + (valid > 0 ? gc : 0),
+                       (int)valid * (int)sizeof(T));
     }
     double* ts = stage_t(st);
     for (int idx = threadIdx.x; idx < b * 16; idx += 256) {
@@ -156,7 +170,7 @@ k_symm_dmma(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
     __syncthreads();                                    // chunk ch landed; stage (ch-1)%S is free
     if (ch + SYMM_STAGES - 1 < chunks) fill(ch + SYMM_STAGES - 1, (ch + SYMM_STAGES - 1) % SYMM_STAGES);
     else asm volatile("cp.async.commit_group;" ::: "memory");
-    const float* ss = stage_s(ch % SYMM_STAGES) + (warp * 32 + fr) * SYMM_SP + fk;
+    const T* ss = stage_s(ch % SYMM_STAGES) + (warp * 32 + fr) * SP + fk;
     const double* ts = stage_t(ch % SYMM_STAGES) + fk;
 #pragma unroll
     for (int ks = 0; ks < SYMM_COLS / 4; ++ks) {
@@ -164,7 +178,7 @@ k_symm_dmma(const float* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
       const double b1 = n1_live ? ts[(8 + fr) * SYMM_TP + 4 * ks] : 0.0;
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
-        const double a = (double)ss[g * 8 * SYMM_SP + 4 * ks];
+        const double a = to_f64(ss[g * 8 * SP + 4 * ks]);
         asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
                      : "+d"(acc[g][0][0]), "+d"(acc[g][0][1]) : "d"(a), "d"(b0));
         if (two_tiles)                                  // b <= 8: the second n-tile would be all zeros
@@ -219,17 +233,18 @@ static size_t block_product_scratch_doubles(int64_t rows, int64_t n, int b, int 
 
 // Y = S T (k_symm_dmma, then k_symm_reduce); `scratch`, `splits` and `cols_per_split` come from
 // block_product_scratch_doubles
-static int launch_block_product(int b, const float* s, int64_t rows, int64_t n, int64_t lds,
+template <typename T>
+static int launch_block_product(int b, const T* s, int64_t rows, int64_t n, int64_t lds,
                                 const double* t, int64_t ldt, double* y, int64_t ldy, double* scratch,
                                 int splits, int64_t cols_per_split, cudaStream_t st) {
   SC_REQUIRE(b >= 1 && b <= SYMM_MAXB && ldt % 2 == 0 && (reinterpret_cast<uintptr_t>(t) & 15) == 0 &&
-             lds % 4 == 0 && (reinterpret_cast<uintptr_t>(s) & 15) == 0,
+             (lds * (int64_t)sizeof(T)) % 16 == 0 && (reinterpret_cast<uintptr_t>(s) & 15) == 0,
              "sc_eigh_extremal: internal (block product alignment)");
   const int row_blocks = (int)((rows + SYMM_ROWS - 1) / SYMM_ROWS);
   const int64_t rows_pad = (rows + 1) & ~(int64_t)1;
   const size_t smem = (size_t)SYMM_STAGES * SYMM_STAGE_BYTES;
-  SC_CUDA(cudaFuncSetAttribute(k_symm_dmma, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_symm_dmma<<<(unsigned)(row_blocks * splits), 256, smem, st>>>(s, rows, n, lds, t, ldt, b, row_blocks,
+  SC_CUDA(cudaFuncSetAttribute(k_symm_dmma<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_symm_dmma<T><<<(unsigned)(row_blocks * splits), 256, smem, st>>>(s, rows, n, lds, t, ldt, b, row_blocks,
                                                                 cols_per_split, scratch, rows_pad);
   sc::launched();
   k_symm_reduce<<<dim3((unsigned)((rows + 255) / 256), (unsigned)b), 256, 0, st>>>(scratch, splits, b, rows,
@@ -671,19 +686,26 @@ typedef int (*sc_gather_fn)(void* user, int count);
 // converged when it is <= tol * max(|theta|max, scale): the complement's spectrum can sit far
 // below the operator's scale (a rank-deficient matrix leaves a cluster of rounding-level values),
 // and relative to the operator's scale is the accuracy its callers need.
-static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t row_begin,
+// Factored operator (sc_eigh_extremal_factored): `s` is NULL and yh = Y (fp16, symmetric) stands
+// for S = Y Y^T; every block product is Y (Y T) through an [b][n] fp64 intermediate, two passes of
+// 2 B per element over Y.
+static int lanczos_impl(sc_context* ctx, const float* s, const __half* yh, int64_t rows,
+                        int64_t row_begin,
                         int64_t n, int64_t lds, const double* delta, const double* left,
                         const double* right, double sign, int which, int64_t n_values,
                         int64_t n_vectors, double tol, int64_t max_matvecs, double* y_ext,
                         int slab, int64_t slab_len, sc_gather_fn gather, void* user,
                         double* locked, int64_t n_locked, double scale,
                         double* w_host, double* v_dev, int64_t* stats_host, void* stream) {
-  SC_REQUIRE(ctx && s && w_host && n > 0, "sc_eigh_extremal: bad arguments");
+  SC_REQUIRE(ctx && (s != nullptr) != (yh != nullptr) && w_host && n > 0,
+             "sc_eigh_extremal: bad arguments");
+  SC_REQUIRE(!yh || (rows == n && y_ext == nullptr), "sc_eigh_extremal: internal (factored operator)");
   SC_REQUIRE(n_values >= 1 && n_values <= 32 && n_vectors >= 0 && n_vectors <= n_values,
              "sc_eigh_extremal: need 1 <= n_values <= 32 and n_vectors <= n_values");
   SC_REQUIRE(n_vectors == 0 || v_dev, "sc_eigh_extremal: v_dev missing");
-  SC_REQUIRE((reinterpret_cast<uintptr_t>(s) & 15) == 0 && lds % 4 == 0,
-             "sc_eigh_extremal: S needs a 16-byte aligned base and lds %% 4 == 0");
+  SC_REQUIRE(s ? ((reinterpret_cast<uintptr_t>(s) & 15) == 0 && lds % 4 == 0)
+               : ((reinterpret_cast<uintptr_t>(yh) & 15) == 0 && lds % 8 == 0),
+             "sc_eigh_extremal: S needs a 16-byte aligned base and lds %% 4 == 0 (Y: lds %% 8 == 0)");
   SC_REQUIRE(n_locked >= 0 && (n_locked == 0 || locked), "sc_eigh_extremal: bad locked set");
   const int nev = (int)n_values;
   const int b = sc_eigh_block_size(n_values);
@@ -701,7 +723,7 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   SC_CUDA(vb.alloc(sizeof(double) * (size_t)jmax * n, st));
   SC_CUDA(vb2.alloc(sizeof(double) * (size_t)jmax * n, st));
   const int64_t ldtb = (n + 1) & ~(int64_t)1;      // even: 16-byte aligned rows for cp.async
-  SC_CUDA(work.alloc(sizeof(double) * (size_t)(ldtb + 2 * n) * b, st));
+  SC_CUDA(work.alloc(sizeof(double) * (size_t)(ldtb + 2 * n + (yh ? ldtb : 0)) * b, st));
   SC_CUDA(small.alloc(sizeof(double) * (size_t)(2 * jmax + 8 + jmax * 64 + 2 * jmax * 16 + 256), st));
   const int bp_chunks = (int)((n + BP_CHUNK - 1) / BP_CHUNK);
   Scratch part;
@@ -718,6 +740,7 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   double* tb = work.as<double>();                  // [b][ldtb] prescaled block
   double* yb = tb + (size_t)b * ldtb;              // [b][n] products (unsharded)
   double* wb = yb + (size_t)b * n;                 // [b][n] Op applied, being orthogonalised
+  double* mid = wb + (size_t)b * n;                // [b][ldtb] Y T of the factored operator
   double* h_dev = small.as<double>();              // [jmax]
   double* h2_dev = h_dev + jmax;                   // [jmax]
   double* nrm_dev = h2_dev + jmax;                 // [1] (+pad)
@@ -868,8 +891,15 @@ static int lanczos_impl(sc_context* ctx, const float* s, int64_t rows, int64_t r
   for (;;) {
     // ---- one pass over S: W = flip * Op V[P..P+b)
     k_prescale<<<dim3(gn, b), 256, 0, st>>>(V + (size_t)P * n, left, right, n, tb, ldtb); sc::launched();
-    if (int rc = launch_block_product(b, s, rows, n, lds, tb, ldtb, y_mine, y_slab_len,
-                                      prod_buf.as<double>(), prod_splits, prod_cols, st)) return rc;
+    if (yh) {
+      if (int rc = launch_block_product(b, yh, rows, n, lds, tb, ldtb, mid, ldtb,
+                                        prod_buf.as<double>(), prod_splits, prod_cols, st)) return rc;
+      if (int rc = launch_block_product(b, yh, rows, n, lds, mid, ldtb, y_mine, y_slab_len,
+                                        prod_buf.as<double>(), prod_splits, prod_cols, st)) return rc;
+    } else if (int rc = launch_block_product(b, s, rows, n, lds, tb, ldtb, y_mine, y_slab_len,
+                                             prod_buf.as<double>(), prod_splits, prod_cols, st)) {
+      return rc;
+    }
     SC_LAUNCH_CHECK();
     if (gather) SC_REQUIRE(gather(user, b) == 0, "sc_eigh_extremal_sharded: the gather callback failed");
     k_postscale<<<dim3(gn, b), 256, 0, st>>>(V + (size_t)P * n, y_base, y_slab_len, b, delta, left,
@@ -1039,9 +1069,39 @@ extern "C" int sc_eigh_extremal(sc_context* ctx, const float* s, int64_t n, int6
                                 double sign, int which, int64_t n_values, int64_t n_vectors,
                                 double tol, int64_t max_matvecs, double* w_host, double* v_dev,
                                 int64_t* stats_host, void* stream) {
-  return lanczos_impl(ctx, s, n, 0, n, lds, delta, left, right, sign, which, n_values, n_vectors,
-                      tol, max_matvecs, nullptr, 0, 0, nullptr, nullptr, nullptr, 0, 0.0, w_host,
-                      v_dev, stats_host, stream);
+  return lanczos_impl(ctx, s, nullptr, n, 0, n, lds, delta, left, right, sign, which, n_values,
+                      n_vectors, tol, max_matvecs, nullptr, 0, 0, nullptr, nullptr, nullptr, 0, 0.0,
+                      w_host, v_dev, stats_host, stream);
+}
+
+extern "C" int sc_eigh_extremal_factored(sc_context* ctx, const void* y_hi, int64_t n, int64_t ldy,
+                                         const double* delta, const double* left,
+                                         const double* right, double sign, int which,
+                                         int64_t n_values, int64_t n_vectors, double tol,
+                                         int64_t max_matvecs, double* w_host, double* v_dev,
+                                         int64_t* stats_host, void* stream) {
+  SC_REQUIRE(y_hi, "sc_eigh_extremal_factored: y_hi missing");
+  return lanczos_impl(ctx, nullptr, (const __half*)y_hi, n, 0, n, ldy, delta, left, right, sign,
+                      which, n_values, n_vectors, tol, max_matvecs, nullptr, 0, 0, nullptr, nullptr,
+                      nullptr, 0, 0.0, w_host, v_dev, stats_host, stream);
+}
+
+extern "C" int sc_block_product_f16(sc_context* ctx, const void* s, int64_t rows, int64_t n,
+                                    int64_t lds, const double* t, int64_t ldt, int b, double* y,
+                                    int64_t ldy, void* stream) {
+  SC_REQUIRE(ctx && s && t && y && rows > 0 && n > 0 && b >= 1 && b <= SYMM_MAXB && ldt >= n && ldy >= rows,
+             "sc_block_product_f16: bad arguments");
+  SC_REQUIRE(lds % 8 == 0 && (reinterpret_cast<uintptr_t>(s) & 15) == 0,
+             "sc_block_product_f16: `s` needs a 16-byte aligned base and lds %% 8 == 0");
+  cudaStream_t st = as_stream(stream);
+  int splits = 1;
+  int64_t cols = n;
+  Scratch buf;
+  SC_CUDA(buf.alloc(sizeof(double) * block_product_scratch_doubles(rows, n, b, ctx->sm_count, &splits, &cols), st));
+  if (int rc = launch_block_product(b, (const __half*)s, rows, n, lds, t, ldt, y, ldy, buf.as<double>(),
+                                    splits, cols, st)) return rc;
+  SC_LAUNCH_CHECK();
+  return 0;
 }
 
 extern "C" int sc_eigh_extremal_locked(sc_context* ctx, const float* s, int64_t n, int64_t lds,
@@ -1051,7 +1111,7 @@ extern "C" int sc_eigh_extremal_locked(sc_context* ctx, const float* s, int64_t 
                                        int64_t n_locked, double* w_host, int64_t* stats_host,
                                        void* stream) {
   SC_REQUIRE(locked, "sc_eigh_extremal_locked: locked buffer missing");
-  return lanczos_impl(ctx, s, n, 0, n, lds, delta, left, right, sign, which, n_values, 0, tol,
+  return lanczos_impl(ctx, s, nullptr, n, 0, n, lds, delta, left, right, sign, which, n_values, 0, tol,
                       max_matvecs, nullptr, 0, 0, nullptr, nullptr, locked, n_locked, scale, w_host,
                       nullptr, stats_host, stream);
 }
@@ -1083,7 +1143,7 @@ extern "C" int sc_eigh_extremal_sharded(sc_context* ctx, const float* s_block, i
              "sc_eigh_extremal_sharded: bad arguments");
   SC_REQUIRE(slab >= 0 && slab_len > 0 && row_begin == (int64_t)slab * slab_len && rows <= slab_len,
              "sc_eigh_extremal_sharded: rank `slab` must own rows [slab*slab_len, +rows)");
-  return lanczos_impl(ctx, s_block, rows, row_begin, n, lds, delta, left, right, sign, which,
+  return lanczos_impl(ctx, s_block, nullptr, rows, row_begin, n, lds, delta, left, right, sign, which,
                       n_values, n_vectors, tol, max_matvecs, y_slabs, slab, slab_len, gather, user,
                       nullptr, 0, 0.0, w_host, v_dev, stats_host, stream);
 }

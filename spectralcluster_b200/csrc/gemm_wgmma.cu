@@ -532,11 +532,12 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
         }
       }
     }
-    // ---- stores: a warp's float2 store covers 8 rows x 32 contiguous bytes
+    // ---- stores: a warp's float2 store covers 8 rows x 32 contiguous bytes.  C == NULL keeps the
+    // row statistics (and a mirrored block) only: nothing of C is written.
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int64_t row = r0 + 8 * h;
-      if (!full && row >= M) continue;
+      if (C == nullptr || (!full && row >= M)) continue;
       float* dst = C + row * ldc + col0;
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
@@ -554,7 +555,7 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
     // the peer's block S(p,g) = S(g,p)^T mapped into this process by CUDA IPC, so that the
     // exchange rides on the GEMM epilogue tile by tile.  Lanes with the same lane % 4 hold 8
     // consecutive rows: every store instruction writes 4 x 32 contiguous bytes.
-    float* tdst = mirror ? C : (!SYM ? mirror_out : nullptr);
+    float* tdst = mirror ? C : (!SYM ? mirror_out : nullptr);   // NULL when C is (stats only)
     const int64_t ldt = mirror ? ldc : ldm;
     if (tdst != nullptr) {
 #pragma unroll
@@ -694,6 +695,7 @@ int gemm_nt_wgmma(const sc_context* ctx, int epi, int precision, const __half* a
                   double* stat_rowsum, float* mirror, int64_t ldm, cudaStream_t st) {
   SC_REQUIRE(M > 0 && N > 0 && K > 0 && M < (1LL << 31) && N < (1LL << 31) && K < (1LL << 31),
              "wgmma GEMM: bad shape");
+  SC_REQUIRE(C || stat_rowmax || mirror, "wgmma GEMM: nothing to write");
   SC_REQUIRE((reinterpret_cast<uintptr_t>(C) & 7) == 0 && ldc % 2 == 0,
              "wgmma GEMM: C needs an 8-byte aligned base and ldc %% 2 == 0");
   SC_REQUIRE(precision == SC_GEMM_SPLIT3 || precision == SC_GEMM_SPLIT2 ||

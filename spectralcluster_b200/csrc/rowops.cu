@@ -42,12 +42,13 @@ __global__ void k_normalize_rows(const T* __restrict__ x, int64_t n, int64_t d, 
 }
 
 // ------------------------------------------------------------------ crop diagonal
-// diag_out (optional) receives the new diagonal; out (optional) the full matrix.
+// diag_out (optional) receives the new diagonal; out (optional) the full matrix.  Row blockIdx.x
+// of `a` is row row0 + blockIdx.x of the matrix (a row panel; row0 = 0 for the whole matrix).
 __global__ void k_crop_diagonal(const float* a, int64_t n, int64_t lda, float* out, int64_t ldo,
-                                float* __restrict__ diag_out) {
+                                float* __restrict__ diag_out, int64_t row0) {
   __shared__ float red[32];
-  const int64_t i = blockIdx.x;
-  const float* r = a + i * lda;
+  const int64_t i = row0 + blockIdx.x;
+  const float* r = a + (int64_t)blockIdx.x * lda;
   float m = 0.0f;  // the zeroed diagonal takes part in the max (refinement.py:148-149)
   // 128-bit loads when the row is 16-byte aligned (every matrix the Python host allocates)
   const bool vec = ((lda & 3) == 0) && ((reinterpret_cast<uintptr_t>(a) & 15) == 0);
@@ -66,9 +67,9 @@ __global__ void k_crop_diagonal(const float* a, int64_t n, int64_t lda, float* o
   for (int64_t j = n4 + threadIdx.x; j < n; j += blockDim.x)
     if (j != i) m = fmaxf(m, r[j]);
   m = block_max(m, red);
-  if (diag_out && threadIdx.x == 0) diag_out[i] = m;
+  if (diag_out && threadIdx.x == 0) diag_out[blockIdx.x] = m;
   if (out) {
-    float* o = out + i * ldo;
+    float* o = out + (int64_t)blockIdx.x * ldo;
     if (out == a) {
       if (threadIdx.x == 0) o[i] = m;
     } else {
@@ -400,6 +401,15 @@ __global__ void k_laplacian(const float* __restrict__ w, int64_t n, int64_t ldw,
   out[i * ldo + j] = (float)v;
 }
 
+// CropDiagonal values of the rows [row_begin, row_begin + rows) held by the panel `a`.
+int crop_diagonal_rows(const float* a, int64_t n, int64_t lda, int64_t row_begin, int64_t rows,
+                       float* diag_out, cudaStream_t st) {
+  k_crop_diagonal<<<(unsigned)rows, 256, 0, st>>>(a, n, lda, nullptr, 0, diag_out, row_begin);
+  sc::launched();
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace sc
 
 // ====================================================================== C ABI
@@ -426,7 +436,7 @@ extern "C" int sc_normalize_rows(sc_context* ctx, const void* x, int x_is_f64, i
 extern "C" int sc_crop_diagonal(sc_context* ctx, const float* a, int64_t n, int64_t lda,
                                 float* out, int64_t ldo, void* stream) {
   SC_REQUIRE(ctx && a && out && n > 0, "sc_crop_diagonal: bad arguments");
-  k_crop_diagonal<<<(unsigned)n, 256, 0, as_stream(stream)>>>(a, n, lda, out, ldo, nullptr); sc::launched();
+  k_crop_diagonal<<<(unsigned)n, 256, 0, as_stream(stream)>>>(a, n, lda, out, ldo, nullptr, 0); sc::launched();
   SC_LAUNCH_CHECK();
   return 0;
 }
@@ -434,7 +444,7 @@ extern "C" int sc_crop_diagonal(sc_context* ctx, const float* a, int64_t n, int6
 extern "C" int sc_crop_diagonal_values(sc_context* ctx, const float* a, int64_t n, int64_t lda,
                                        float* diag_out, void* stream) {
   SC_REQUIRE(ctx && a && diag_out && n > 0, "sc_crop_diagonal_values: bad arguments");
-  k_crop_diagonal<<<(unsigned)n, 256, 0, as_stream(stream)>>>(a, n, lda, nullptr, 0, diag_out); sc::launched();
+  k_crop_diagonal<<<(unsigned)n, 256, 0, as_stream(stream)>>>(a, n, lda, nullptr, 0, diag_out, 0); sc::launched();
   SC_LAUNCH_CHECK();
   return 0;
 }

@@ -28,6 +28,42 @@ _torch = None
 # needs three below (the parity tests pin these sizes).
 AUTO_SINGLE_FROM, AUTO_SPLIT2_FROM = 16384, 4096
 
+# The stored route keeps about this many bytes per element of the N x ld matrices alive at its
+# peak: A and B (fp32) while the blur writes Y (fp16 hi plane), then S (fp32) beside A and Y.
+STORED_ROUTE_BYTES_PER_ELEMENT = 10
+# Device memory the route choice leaves for the CUDA context, the allocator and the vectors.
+FACTORED_ROUTE_RESERVE = 4 << 30
+# The factored route builds the affinity and the blur in row panels of about this many bytes.
+FACTORED_PANEL_BYTES = 1 << 30
+# Panel origins sit on the affinity's 128-row tiles (which also aligns them with the 64-row tiles
+# of the threshold pass and the 32-row bands of the blur); the blur reads 4 rows on either side.
+PANEL_ALIGN, BLUR_HALO = 128, 4
+
+
+def stored_route_peak_bytes(n: int) -> int:
+  """Peak device bytes of predict()'s stored route at n, computed from shapes."""
+  return STORED_ROUTE_BYTES_PER_ELEMENT * n * round_up(n, 64)
+
+
+def panel_rows_for(n: int) -> int:
+  """Rows per panel of the factored route: about FACTORED_PANEL_BYTES of fp32 rows, a multiple of
+  PANEL_ALIGN, chosen from n alone."""
+  rows = FACTORED_PANEL_BYTES // (4 * round_up(n, 64)) // PANEL_ALIGN * PANEL_ALIGN
+  return max(PANEL_ALIGN, min(rows, round_up(n, PANEL_ALIGN)))
+
+
+def panel_plan(n: int, rows: int):
+  """[(r0, r1, a0, a1)]: the factored route's panels produce the rows [r0, r1) (every row once,
+  r0 a multiple of `rows`) from the affinity rows [a0, a1) = the blur halo [r0 - 4, r1 + 4) clipped
+  at 0 and n, with a0 moved down to a multiple of PANEL_ALIGN."""
+  assert rows > 0 and rows % PANEL_ALIGN == 0
+  plan = []
+  for r0 in range(0, n, rows):
+    r1 = min(n, r0 + rows)
+    a0 = max(0, r0 - BLUR_HALO) // PANEL_ALIGN * PANEL_ALIGN
+    plan.append((r0, r1, a0, min(n, r1 + BLUR_HALO)))
+  return plan
+
 
 def torch():
   global _torch
@@ -74,6 +110,12 @@ class Engine:
     # Diffuse inside predict() (K = N): an sc_gemm_precision to use at every N, or None for the
     # N-based policy above.  The operator-level API (refinement.Diffuse) always uses split3.
     self.diffuse_precision = None
+    # predict() takes the factored route (no N x N fp32 matrix) when the stored route's peak,
+    # stored_route_peak_bytes(n), exceeds this many bytes and the call is within its scope.
+    # Computed from the device's total memory, never from what is free, so that one GPU model
+    # always takes the same route for the same call.
+    self.factored_above_bytes = (t.cuda.get_device_properties(device).total_memory -
+                                 FACTORED_ROUTE_RESERVE)
     self.profile = None
 
   @classmethod
@@ -316,6 +358,66 @@ class Engine:
               hi.stride(0), n, _ptr(s), s.stride(0), _ptr(mx), _ptr(sm), self.stream)
     return s, mx, sm
 
+  def diffuse_stats(self, n, hi):
+    """(rowmax fp32, rowsum fp64) of S = Y Y^T from the single-MMA Diffuse on the hi plane of Y,
+    without storing S (bitwise the statistics of the storing call)."""
+    t = torch()
+    mx, sm = self.vector(n, t.float32), self.vector(n, t.float64)
+    self.call("sc_diffuse", nat.GEMM_TCGEN05, nat.GEMM_SINGLE, None, 0, _ptr(hi), None,
+              hi.stride(0), n, None, 0, _ptr(mx), _ptr(sm), self.stream)
+    return mx, sm
+
+  # ---- row panels of the factored route
+  def normalized_planes(self, x_dev):
+    """Split fp16 planes of the row-normalised embeddings (the affinity GEMM's operands)."""
+    t = torch()
+    n, d = int(x_dev.shape[0]), int(x_dev.shape[1])
+    hi, lo = self.planes(n, d)
+    self.call("sc_normalize_rows", _ptr(x_dev), 1 if x_dev.dtype == t.float64 else 0, n, d,
+              x_dev.stride(0), None, 0, _ptr(hi), _ptr(lo), hi.stride(0), self.stream)
+    return hi, lo
+
+  def affinity_panel(self, hi, lo, n, d, a0, a1, crop=None):
+    """Rows [a0, a1) of the affinity (bitwise those of affinity()); with `crop` (fp32, length n)
+    their CropDiagonal values also land in crop[a0:a1]."""
+    t = torch()
+    panel = t.empty((a1 - a0, round_up(n, 64)), dtype=t.float32, device=self.device)
+    self.call("sc_affinity_cosine_panel", self.gemm_precision, _ptr(hi), _ptr(lo), hi.stride(0),
+              n, d, a0, a1 - a0, _ptr(panel), panel.stride(0),
+              None if crop is None else _ptr(crop[a0:]), self.stream)
+    return panel
+
+  def blur_upper_rowmax_block(self, panel, a0, n, r0, r1, sigma, diag, zero_diag, b, m):
+    """Pass 1 of the symmetric blur pair on a panel: b <- upper tiles of rows [r0, r1), and their
+    row and column maxima folded into m."""
+    self.call("sc_blur_upper_rowmax_block", _ptr(panel), n, panel.stride(0), a0,
+              int(panel.shape[0]), r0, r1, _ptr(diag), float(sigma), int(bool(zero_diag)), _ptr(b),
+              b.stride(0), _ptr(m), self.stream)
+
+  def threshold_symmetrize_upper_block(self, b, n, r0, r1, rowmax, p, mult, binarize,
+                                       preserve_diag, sym_type, hi):
+    """Pass 2 on a panel: Y_hi (full size) <- the tile pairs whose rows lie in [r0, r1)."""
+    self.call("sc_threshold_symmetrize_upper_block", _ptr(b), n, b.stride(0), r0, r1,
+              _ptr(rowmax), float(p), float(mult), int(bool(binarize)), int(bool(preserve_diag)),
+              int(sym_type), None, 0, _ptr(hi), None, hi.stride(0), self.stream)
+
+  def block_product_f16(self, s, rows, n, t_, b, y):
+    self.call("sc_block_product_f16", _ptr(s), rows, n, s.stride(0), _ptr(t_), t_.stride(0), b,
+              _ptr(y), y.stride(0), self.stream)
+
+  def eigh_factored(self, y_hi, n, delta, left, right, sign, which, n_values, n_vectors, tol=1e-9,
+                    max_matvecs=0):
+    """eigh() of the block Lanczos solver on S = Y_hi Y_hi^T, S never formed."""
+    t = torch()
+    w = np.empty(max(n_values, 1), dtype=np.float64)
+    v = t.empty((n, max(n_vectors, 1)), dtype=t.float64, device=self.device)
+    stats = np.zeros(4, dtype=np.int64)
+    self.call("sc_eigh_extremal_factored", _ptr(y_hi), n, y_hi.stride(0), _ptr(delta), _ptr(left),
+              _ptr(right), float(sign), int(which), n_values, n_vectors, float(tol),
+              int(max_matvecs), w.ctypes.data_as(ctypes.c_void_p), _ptr(v),
+              stats.ctypes.data_as(ctypes.c_void_p), self.stream)
+    return w[:n_values], v[:, :n_vectors], stats
+
   def row_stats(self, a, n, want_max=True, want_sum=True):
     mx = self.vector(n) if want_max else None
     sm = self.vector(n) if want_sum else None
@@ -493,14 +595,95 @@ class Engine:
 class Refined:
   """Result of the refinement sequence in the structured form the eigensolver wants:
   the matrix is diag(row_scale) * S with S fp32 on the device (`row_scale` None = ones).
-  `symmetric` tells whether S is symmetric (up to rounding)."""
+  `symmetric` tells whether S is symmetric (up to rounding).  On the factored route S is not
+  stored: `s` is None and S = y_hi y_hi^T with y_hi the fp16 hi plane of Y."""
 
-  def __init__(self, s, n, symmetric, row_scale=None, rowsum=None):
+  def __init__(self, s, n, symmetric, row_scale=None, rowsum=None, y_hi=None):
     self.s = s
     self.n = n
     self.symmetric = symmetric
     self.row_scale = row_scale
     self.rowsum = rowsum      # fp64 row sums of S when the Diffuse epilogue produced them
+    self.y_hi = y_hi
+
+
+def factored_sequence_ok(eng: Engine, options) -> bool:
+  """Whether options.refinement_sequence is [CropDiagonal] GaussianBlur RowWiseThreshold(RowMax)
+  Symmetrize Diffuse [RowWiseNormalize] with a radius-4 blur: the chain the factored route runs."""
+  from . import refinement as rf
+  RN = rf.RefinementName
+  names = list(options.refinement_sequence or [])
+  if names[:1] == [RN.CropDiagonal]:
+    names = names[1:]
+  if names[-1:] == [RN.RowWiseNormalize]:
+    names = names[:-1]
+  return (names == [RN.GaussianBlur, RN.RowWiseThreshold, RN.Symmetrize, RN.Diffuse] and
+          options.thresholding_type == rf.ThresholdType.RowMax and
+          isinstance(options.symmetrize_type, rf.SymmetrizeType) and
+          eng.upper_pass_ok(float(options.gaussian_blur_sigma)))
+
+
+class FactoredAffinity:
+  """The affinity of the factored route: never stored, rebuilt in row panels from the split planes
+  of the normalised embeddings.  The blur's row maxima m do not depend on p_percentile, so pass 1
+  runs once per predict() and every AutoTune evaluation reuses it."""
+
+  def __init__(self, eng: Engine, x_dev, panel_rows: typing.Optional[int] = None):
+    self.n, self.d = int(x_dev.shape[0]), int(x_dev.shape[1])
+    self.hi, self.lo = eng.normalized_planes(x_dev)
+    self.panel_rows = panel_rows or panel_rows_for(self.n)
+    self.symmetric = True
+    self.crop_vector = None
+    self._m = None
+
+  def _panels(self, eng: Engine, options):
+    """Yield (r0, r1, affinity panel, its first row a0, crop values by global row or None,
+    B panel) over panel_plan()."""
+    from . import refinement as rf
+    t = torch()
+    crop_first = list(options.refinement_sequence or [])[:1] == [rf.RefinementName.CropDiagonal]
+    diag = eng.vector(self.n, t.float32) if crop_first else None
+    b = t.empty((self.panel_rows, round_up(self.n, 64)), dtype=t.float32, device=eng.device)
+    for r0, r1, a0, a1 in panel_plan(self.n, self.panel_rows):
+      panel = eng.affinity_panel(self.hi, self.lo, self.n, self.d, a0, a1, diag)
+      yield r0, r1, panel, a0, diag, b
+      del panel
+
+  def rowmax(self, eng: Engine, options):
+    """m of the symmetric blur pair (pass 1 over every panel), computed once."""
+    if self._m is None:
+      m = eng.vector(self.n, torch().float32, zero=True)
+      zero_diag = bool(options.thresholding_preserve_diagonal)
+      sigma = float(options.gaussian_blur_sigma)
+      for r0, r1, panel, a0, diag, b in self._panels(eng, options):
+        eng.blur_upper_rowmax_block(panel, a0, self.n, r0, r1, sigma, diag, zero_diag, b, m)
+      self._m = m
+    return self._m
+
+  def refine(self, eng: Engine, options) -> Refined:
+    """The refinement sequence on the factored route: Y_hi by pass 2 over every panel, then the
+    statistics-only Diffuse."""
+    from . import refinement as rf
+    t = torch()
+    n = self.n
+    m = self.rowmax(eng, options)
+    scratch = eng.vector(n, t.float32, zero=True)   # pass 2 re-folds maxima that are already in m
+    y_hi = t.empty((n, round_up(n, 64)), dtype=t.float16, device=eng.device)
+    sym_type = (nat.SYMMETRIZE_MAX if options.symmetrize_type == rf.SymmetrizeType.Max
+                else nat.SYMMETRIZE_AVERAGE)
+    zero_diag = bool(options.thresholding_preserve_diagonal)
+    sigma = float(options.gaussian_blur_sigma)
+    for r0, r1, panel, a0, diag, b in self._panels(eng, options):
+      eng.blur_upper_rowmax_block(panel, a0, n, r0, r1, sigma, diag, zero_diag, b, scratch)
+      eng.threshold_symmetrize_upper_block(
+          b, n, r0, r1, m, options.p_percentile, options.thresholding_soft_multiplier,
+          options.thresholding_with_binarization, zero_diag, sym_type, y_hi)
+    del scratch
+    mx, sm = eng.diffuse_stats(n, y_hi)
+    names = list(options.refinement_sequence)
+    row_scale = 1.0 / mx.double() if names[-1] == rf.RefinementName.RowWiseNormalize else None
+    return Refined(None, n, True, row_scale, sm, y_hi=y_hi)
+
 
 
 def run_refinement(eng: Engine, a, n: int, options, crop_vector=None, a_symmetric=True,

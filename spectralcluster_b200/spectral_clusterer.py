@@ -128,10 +128,13 @@ class SpectralClusterer:
   def _eigen_on_device(self, eng, affinity: DeviceAffinity, constraint_matrix=None):
     """Refinement + Laplacian terms + eigensolve; returns (w host, V device [n, nv], k, gap)."""
     n = affinity.n
-    refined = dev.run_refinement(eng, affinity.matrix, n, self.refinement_options,
-                                 crop_vector=affinity.crop_vector,
-                                 a_symmetric=affinity.symmetric,
-                                 diffuse_precision=eng.diffuse_precision_for(n))
+    if isinstance(affinity, dev.FactoredAffinity):
+      refined = affinity.refine(eng, self.refinement_options)
+    else:
+      refined = dev.run_refinement(eng, affinity.matrix, n, self.refinement_options,
+                                   crop_vector=affinity.crop_vector,
+                                   a_symmetric=affinity.symmetric,
+                                   diffuse_precision=eng.diffuse_precision_for(n))
     if (self.constraint_options and not self.constraint_options.apply_before_refinement and
         constraint_matrix is not None):
       # constraint on the refined affinity (spectral_clusterer.py:137-142)
@@ -164,6 +167,13 @@ class SpectralClusterer:
       else:
         w, v, stats = arnoldi.eig_extremal_device(eng, *op, not descend, limit, n_vectors)
         top_solve = lambda: arnoldi.eig_extremal_device(eng, *op, False, 1, 0)[0]
+    elif refined.y_hi is not None:
+      # factored route (its scope guarantees lanczos_fits): S = Y_hi Y_hi^T is never stored
+      solver = "lanczos-factored"
+      fop = (refined.y_hi,) + op[1:]
+      w, v, stats = eng.eigh_factored(*fop, which, limit, n_vectors)
+      stats = stats.tolist()
+      top_solve = lambda: eng.eigh_factored(*fop, nat.EIG_LARGEST, 1, 0)[0]
     elif n > eng.dense_eig_max and lanczos_fits(n, limit):
       solver = "lanczos"
       w, v, stats = eng.eigh(*op, which, limit, n_vectors, False)
@@ -207,6 +217,23 @@ class SpectralClusterer:
                              solver=solver, lanczos_stats=stats)
     return w, v, k, gap
 
+  def _factored_route(self, eng, n: int, constraint_matrix=None) -> bool:
+    """Whether predict() on n embeddings takes the factored route: the stored route's peak
+    (computed from shapes) exceeds eng.factored_above_bytes and every option is one the factored
+    route serves; any other call keeps the stored route."""
+    if dev.stored_route_peak_bytes(n) <= eng.factored_above_bytes:
+      return False
+    limit = (self.max_clusters or 0) + 1
+    return (self.affinity_function is utils.compute_affinity_matrix and
+            self.min_clusters != 1 and (self.min_clusters or 0) <= limit and
+            not (self.constraint_options and constraint_matrix is not None) and
+            self.max_clusters is not None and self.max_clusters < LANCZOS_MAX_PAIRS and
+            n > limit and n > eng.dense_eig_max and lanczos_fits(n, limit) and
+            self.autotune_group is None and
+            eng.gemm_engine(n) == nat.GEMM_TCGEN05 and
+            eng.diffuse_precision_for(n) == nat.GEMM_SINGLE and
+            dev.factored_sequence_ok(eng, self.refinement_options))
+
   def _count_clusters(self, eigenvalues, descend: bool, max_eigenvalue=None):
     """utils.compute_number_of_clusters with this clusterer's options -> (k, max gap); only a
     descending spectrum stops at stop_eigenvalue.  `max_eigenvalue`: lambda_max of a spectrum of
@@ -223,7 +250,7 @@ class SpectralClusterer:
     back as a host ndarray [n, n_vec] in the first case, a device fp64 tensor in the second;
     n_vec covers every column predict() can select (all n when max_clusters is None)."""
     eng = dev.Engine.get()
-    if isinstance(affinity, DeviceAffinity):
+    if isinstance(affinity, (DeviceAffinity, dev.FactoredAffinity)):
       _, v, k, gap = self._eigen_on_device(eng, affinity, constraint_matrix)
       return v, k, gap
     a = np.asarray(affinity)
@@ -279,7 +306,13 @@ class SpectralClusterer:
     eng = dev.Engine.get()
     t = dev.torch()
     sequence = list(self.refinement_options.refinement_sequence or [])
-    if self.affinity_function is utils.compute_affinity_matrix:
+    if self._factored_route(eng, num_embeddings, constraint_matrix):
+      x = np.ascontiguousarray(embeddings)
+      if x.dtype not in (np.float32, np.float64):
+        x = x.astype(np.float64)
+      x_dev = t.from_numpy(x).to(eng.device, non_blocking=True)
+      affinity = dev.FactoredAffinity(eng, x_dev)
+    elif self.affinity_function is utils.compute_affinity_matrix:
       x = np.ascontiguousarray(embeddings)
       if x.dtype not in (np.float32, np.float64):
         x = x.astype(np.float64)
