@@ -332,6 +332,19 @@ int sc_eigh_extremal_sharded(sc_context* ctx, const float* s_block, int64_t rows
                              int slab, int64_t slab_len, sc_gather_fn gather, void* user,
                              double* w_host, double* v_dev, int64_t* stats_host, void* stream);
 
+/* One window of a windowed solve on a row-sharded S: sc_eigh_extremal_locked with the row block,
+ * slabs and gather callback of sc_eigh_extremal_sharded.  locked[0..n_locked) is full length and
+ * replicated on every rank (the deflation runs on the gathered products); the window's Ritz
+ * vectors are appended at locked[n_locked..), identically on every rank.  SYNCHRONOUS. */
+int sc_eigh_extremal_locked_sharded(sc_context* ctx, const float* s_block, int64_t rows,
+                                    int64_t row_begin, int64_t n, int64_t lds, const double* delta,
+                                    const double* left, const double* right, double sign,
+                                    int which, int64_t n_values, double tol, int64_t max_matvecs,
+                                    double scale, double* locked, int64_t n_locked,
+                                    double* y_slabs, int slab, int64_t slab_len,
+                                    sc_gather_fn gather, void* user, double* w_host,
+                                    int64_t* stats_host, void* stream);
+
 /* The block product of the extremal solver on its own (the O(N^2) part of what replaces
  * np.linalg.eig at utils.py:59): y[p][0..rows) = s[0..rows, 0..n) t[p][0..n) for p < b <= 16; `s` fp32
  * row-major (16-byte aligned, lds % 4 == 0), `t` / `y` fp64 vector-major with leading dimensions

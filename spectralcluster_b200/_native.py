@@ -85,6 +85,10 @@ PROTOTYPES = {
     "sc_eigh_extremal_sharded": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr,
                                  c_dbl, c_int, c_i64, c_i64, c_dbl, c_i64, c_ptr, c_int, c_i64,
                                  c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_eigh_extremal_locked_sharded": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr,
+                                        c_ptr, c_dbl, c_int, c_i64, c_dbl, c_i64, c_dbl, c_ptr,
+                                        c_i64, c_ptr, c_int, c_i64, c_ptr, c_ptr, c_ptr, c_ptr,
+                                        c_ptr],
     "sc_block_product": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, ctypes.c_int, c_ptr, c_i64,
                          c_ptr],
     "sc_block_product_f16": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, ctypes.c_int, c_ptr,

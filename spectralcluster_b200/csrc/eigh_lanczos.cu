@@ -1148,6 +1148,27 @@ extern "C" int sc_eigh_extremal_sharded(sc_context* ctx, const float* s_block, i
                       nullptr, 0, 0.0, w_host, v_dev, stats_host, stream);
 }
 
+// One window of the windowed solve on a row-sharded S.  The locked set is full length and
+// replicated on every rank: its deflation runs on the gathered products, like the rest of the
+// O(n m b) vector work, so only the block product reads the local rows.
+extern "C" int sc_eigh_extremal_locked_sharded(sc_context* ctx, const float* s_block, int64_t rows,
+                                               int64_t row_begin, int64_t n, int64_t lds,
+                                               const double* delta, const double* left,
+                                               const double* right, double sign, int which,
+                                               int64_t n_values, double tol, int64_t max_matvecs,
+                                               double scale, double* locked, int64_t n_locked,
+                                               double* y_slabs, int slab, int64_t slab_len,
+                                               sc_gather_fn gather, void* user, double* w_host,
+                                               int64_t* stats_host, void* stream) {
+  SC_REQUIRE(s_block && y_slabs && gather && locked && rows > 0 && row_begin >= 0 &&
+             row_begin + rows <= n, "sc_eigh_extremal_locked_sharded: bad arguments");
+  SC_REQUIRE(slab >= 0 && slab_len > 0 && row_begin == (int64_t)slab * slab_len && rows <= slab_len,
+             "sc_eigh_extremal_locked_sharded: rank `slab` must own rows [slab*slab_len, +rows)");
+  return lanczos_impl(ctx, s_block, nullptr, rows, row_begin, n, lds, delta, left, right, sign, which,
+                      n_values, 0, tol, max_matvecs, y_slabs, slab, slab_len, gather, user, locked,
+                      n_locked, scale, w_host, nullptr, stats_host, stream);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Krylov primitives for the GENERAL (non-symmetrisable) eigen path (SURVEY.md 8(f)-1;
 // utils.py:59-61 is np.linalg.eig + .real).  The N-length work -- products with the fp32 matrix,

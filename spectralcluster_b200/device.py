@@ -184,6 +184,7 @@ class Engine:
       "sc_eigh_extremal": "utils.compute_sorted_eigenvectors",
       "sc_eigh_extremal_sharded": "utils.compute_sorted_eigenvectors",
       "sc_eigh_extremal_locked": "utils.compute_sorted_eigenvectors",
+      "sc_eigh_extremal_locked_sharded": "utils.compute_sorted_eigenvectors",
       "sc_eigh_mapback": "utils.compute_sorted_eigenvectors",
       "sc_kmeans": "custom_distance_kmeans.run_kmeans", "sc_row_renorm": "spectral_clusterer.row_wise_renorm",
       "sc_affinity_stats": "fallback_clusterer.check_single_cluster",

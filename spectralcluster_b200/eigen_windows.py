@@ -32,6 +32,17 @@ WINDOW_PAIRS = 16             # eigenpairs per window: one 16-vector block produ
 MAX_WINDOW_PAIRS = 512        # most eigenpairs a windowed solve finds before it gives up
 SETTLE_RTOL = 1e-5            # relative eigenvalue tolerance: a near tie asks for another window
 GROW_START, GROW_CAP = 16, 256   # Krylov-Schur pairs: first solve, most before it gives up
+# Lanczos basis of one window (sc_eigh_extremal_locked*): a 16-vector block, six blocks processed
+# before a thick restart plus the block being processed.  A window needs
+# n - (vectors already locked) >= 2 x this basis.
+WINDOW_BASIS = 7 * WINDOW_PAIRS
+
+
+def capacity(n: int, max_clusters, min_clusters) -> int:
+  """Rows of the locked set of a windowed solve: the eigenvalues it may need (all n when
+  max_clusters is None, capped at MAX_WINDOW_PAIRS), plus one window that may overshoot them."""
+  limit = min(n, max_clusters + 1) if max_clusters else n
+  return min(n, MAX_WINDOW_PAIRS, max(limit, min_clusters or 0) + WINDOW_PAIRS)
 
 
 def settled(prefix, descend: bool, max_clusters: typing.Optional[int], stop_eigenvalue: float,

@@ -25,6 +25,7 @@ ABI; the CPU tests plug in a NumPy backend and run the same code under gloo with
 
 from __future__ import annotations
 
+import ctypes
 import math
 import typing
 
@@ -527,13 +528,105 @@ class DeviceBackend:
     return mx, sm
 
 
+class ShardedOps:
+  """The eigensolver on a row-sharded S: the operator diag(delta) + sign * diag(left) S diag(right)
+  with this rank's row block of S.  Every block product streams the local rows and all-gathers the
+  slabs (b N doubles per pass over S); everything else -- Gram-Schmidt, the locked set, the Ritz
+  pairs -- runs replicated on full-length vectors, so every rank returns bitwise identical values.
+
+  extremal() is one sc_eigh_extremal_sharded solve.  window / lambda_max / vectors are the ops
+  eigen_windows.solve drives, as eigen_windows.DeviceOps on one GPU; their locked set of
+  `capacity` full-length vectors is replicated on every rank."""
+
+  def __init__(self, eng, s_block, plan, n, delta, left, right, sign, which, width: int,
+               dist=None, group=None, capacity: int = 0):
+    from . import _native as nat
+    from . import device as dev
+    t = dev.torch()
+    self.eng, self.nat, self.ptr = eng, nat, dev._ptr
+    self.s_block, self.plan, self.n = s_block, plan, n
+    self.delta, self.left, self.right, self.sign, self.which = delta, left, right, sign, which
+    world, rank = plan.world, plan.rank
+    # block products land in slabs [rank][vector][block]: one all-gather of contiguous slabs per
+    # pass over S completes all `width` (or fewer) vectors on every rank
+    y_slabs = t.zeros((world * width * plan.block,), dtype=t.float64, device=eng.device)
+
+    def gather(_user, count):
+      try:
+        if world > 1:
+          per = count * plan.block
+          dist.all_gather_into_tensor(y_slabs[:world * per], y_slabs[rank * per:(rank + 1) * per].clone(),
+                                      group=group)
+        return 0
+      except Exception:                                  # never unwind through the C frame
+        return 1
+
+    self.y_slabs, self.callback = y_slabs, nat.GATHER_FN(gather)
+    self.locked = t.empty((capacity, n), dtype=t.float64, device=eng.device) if capacity else None
+    self.count, self.scale = 0, 0.0
+    self.stats = dict(windows=0, passes=0, matvecs=0, restarts=0)
+
+  def _slab_args(self):
+    return (self.ptr(self.y_slabs), self.plan.rank, self.plan.block, self.callback, None)
+
+  def extremal(self, which, n_values, n_vectors):
+    """The n_values extremal eigenvalues (host fp64), eigenvectors for the first n_vectors of
+    them (device fp64 [n, n_vectors]) and the solver's stats[4]."""
+    from . import device as dev
+    t = dev.torch()
+    s, plan, ptr = self.s_block, self.plan, self.ptr
+    w = np.empty(n_values, dtype=np.float64)
+    v = t.empty((self.n, n_vectors), dtype=t.float64, device=self.eng.device)
+    stats = np.zeros(4, dtype=np.int64)
+    self.eng.call("sc_eigh_extremal_sharded", ptr(s), plan.rows, plan.row_begin, self.n,
+                  s.stride(0), ptr(self.delta), ptr(self.left), ptr(self.right), float(self.sign),
+                  int(which), n_values, n_vectors, 1e-9, 0, *self._slab_args(),
+                  w.ctypes.data_as(ctypes.c_void_p), ptr(v) if n_vectors else None,
+                  stats.ctypes.data_as(ctypes.c_void_p), self.eng.stream)
+    return w, v, stats
+
+  def window(self, count):
+    s, plan, ptr = self.s_block, self.plan, self.ptr
+    assert self.count + count <= self.locked.shape[0]
+    w = np.empty(count, dtype=np.float64)
+    st = np.zeros(4, dtype=np.int64)
+    self.eng.call("sc_eigh_extremal_locked_sharded", ptr(s), plan.rows, plan.row_begin, self.n,
+                  s.stride(0), ptr(self.delta), ptr(self.left), ptr(self.right), float(self.sign),
+                  int(self.which), count, 1e-9, 0, float(self.scale), ptr(self.locked), self.count,
+                  *self._slab_args(), w.ctypes.data_as(ctypes.c_void_p),
+                  st.ctypes.data_as(ctypes.c_void_p), self.eng.stream)
+    self.count += count
+    self.scale = max(self.scale, float(np.abs(w).max()))
+    self.stats["windows"] += 1
+    self.stats["matvecs"] += int(st[0])
+    self.stats["restarts"] += int(st[1])
+    self.stats["passes"] += int(st[3])
+    return w
+
+  def lambda_max(self):
+    w, _, st = self.extremal(self.nat.EIG_LARGEST, 1, 0)
+    self.scale = max(self.scale, abs(float(w[0])))
+    self.stats["passes"] += int(st[3])
+    return float(w[0])
+
+  def vectors(self, cols):
+    return self.eng.eigh_mapback(self.locked, self.n, cols, self.left, self.right)
+
+
+def windowed(clusterer) -> bool:
+  """Whether predict_sharded() solves in windows: max_clusters None or more pairs than one
+  Lanczos solve finds."""
+  from .spectral_clusterer import LANCZOS_MAX_PAIRS
+  return not clusterer.max_clusters or clusterer.max_clusters + 1 > LANCZOS_MAX_PAIRS
+
+
 def check_sharded_options(clusterer, num_embeddings: int):
   """The argument / option checks of predict() that also apply to predict_sharded(): a clusterer
   configured with something this path does not implement must fail here, not silently return
   labels that differ from predict() and from the reference."""
   from . import custom_distance_kmeans, utils
-  if clusterer.autotune or not clusterer.max_clusters:
-    raise NotImplementedError("predict_sharded: needs max_clusters and no AutoTune")
+  if clusterer.autotune:
+    raise NotImplementedError("predict_sharded: AutoTune is not sharded")
   if clusterer.affinity_function is not utils.compute_affinity_matrix:
     raise NotImplementedError("predict_sharded: only the built-in cosine affinity is sharded")
   if num_embeddings < clusterer.fallback_options.spectral_min_embeddings:
@@ -545,13 +638,23 @@ def check_sharded_options(clusterer, num_embeddings: int):
     raise NotImplementedError("predict_sharded: single-cluster detection is not sharded")
   if clusterer.constraint_options:
     raise NotImplementedError("predict_sharded: constraints are not sharded")
-  from .spectral_clusterer import LANCZOS_MAX_PAIRS, lanczos_basis, lanczos_fits
-  limit = clusterer.max_clusters + 1
-  if limit > LANCZOS_MAX_PAIRS:
-    raise NotImplementedError("predict_sharded: max_clusters <= 31 (extremal eigensolver)")
-  if not lanczos_fits(num_embeddings, limit):
-    raise ValueError("predict_sharded: n=%d is too small for the Lanczos basis (%d vectors); "
-                     "use predict()" % (num_embeddings, lanczos_basis(limit)))
+  from . import eigen_windows as ew
+  from .spectral_clusterer import lanczos_basis, lanczos_fits
+  if not windowed(clusterer):
+    limit = clusterer.max_clusters + 1
+    if not lanczos_fits(num_embeddings, limit):
+      raise ValueError("predict_sharded: n=%d is too small for the Lanczos basis (%d vectors); "
+                       "use predict()" % (num_embeddings, lanczos_basis(limit)))
+    return
+  if clusterer.max_clusters and clusterer.max_clusters + 1 > ew.MAX_WINDOW_PAIRS:
+    raise ew._cap_error(clusterer.max_clusters, ew.MAX_WINDOW_PAIRS)
+  # the last window starts with up to capacity - WINDOW_PAIRS vectors locked
+  capacity = ew.capacity(num_embeddings, clusterer.max_clusters, clusterer.min_clusters)
+  locked = max(capacity - ew.WINDOW_PAIRS, 0)
+  if num_embeddings - locked < 2 * ew.WINDOW_BASIS:
+    raise ValueError("predict_sharded: n=%d is too small for the windowed Lanczos basis (%d "
+                     "locked + %d vectors); use predict()"
+                     % (num_embeddings, locked, 2 * ew.WINDOW_BASIS))
 
 
 def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
@@ -562,9 +665,10 @@ def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
 
   Refinement as in ShardedRefiner; row maxima / sums all-gathered (2 N doubles); eigensolve by the
   sharded thick-restart Lanczos (each matvec streams the local row block and all-gathers N
-  doubles); eigengap and k-means replicated on the [N, k] eigenvectors."""
-  import ctypes
+  doubles), in windows with a replicated locked set when max_clusters is None or >= 32; eigengap
+  and k-means replicated on the [N, k] eigenvectors."""
   from . import _native as nat
+  from . import eigen_windows as ew
   from . import custom_distance_kmeans, device as dev, laplacian as lap, utils
   from . import refinement as rf
   t = dev.torch()
@@ -606,41 +710,38 @@ def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
   normalized = list(opt.refinement_sequence)[-1] == rf.RefinementName.RowWiseNormalize
   r = (1.0 / rowmax) if normalized else None
   delta, left, right, sign, which = lap.terms_from_row_sums(rowsum, r, clusterer.laplacian_type)
-  limit = min(n, clusterer.max_clusters + 1)
-  n_vectors = min(n, max(limit, clusterer.min_clusters or 0))
-  w = np.empty(limit, dtype=np.float64)
-  v = t.empty((n, n_vectors), dtype=t.float64, device=eng.device)
-  stats = np.zeros(4, dtype=np.int64)
-  # block products land in slabs [rank][vector][block]: one all-gather of contiguous slabs per
-  # pass over S completes all b vectors on every rank
-  width = int(nat.load().sc_eigh_block_size(limit))
-  y_slabs = t.zeros((world * width * plan.block,), dtype=t.float64, device=eng.device)
-
-  def gather(_user, count):
-    try:
-      if world > 1:
-        per = count * plan.block
-        dist.all_gather_into_tensor(y_slabs[:world * per], y_slabs[rank * per:(rank + 1) * per].clone(),
-                                    group=group)
-      return 0
-    except Exception:                                  # never unwind through the C frame
-      return 1
-
-  callback = nat.GATHER_FN(gather)
-  s_block = res["s_block"]
-  eng.call("sc_eigh_extremal_sharded", dev._ptr(s_block), plan.rows, plan.row_begin, n,
-           s_block.stride(0), dev._ptr(delta), dev._ptr(left), dev._ptr(right), float(sign),
-           int(which), limit, n_vectors, 1e-9, 0, dev._ptr(y_slabs), rank, plan.block, callback,
-           None, w.ctypes.data_as(ctypes.c_void_p), dev._ptr(v),
-           stats.ctypes.data_as(ctypes.c_void_p), eng.stream)
   descend = which == nat.EIG_LARGEST
-  if not descend and clusterer.eigengap_type == utils.EigenGapType.NormalizedDiff:
-    raise NotImplementedError("predict_sharded: NormalizedDiff on a Laplacian needs lambda_max")
-  k, gap = clusterer._count_clusters(w, descend)
-  clusterer.last_details = dict(eigenvalues=w.copy(), n_clusters_raw=k, max_gap=gap,
-                                solver="lanczos-sharded x%d" % world,
+  op = (eng, res["s_block"], plan, n, delta, left, right, sign, which)
+  dist_args = dict(dist=dist if world > 1 else None, group=group)
+  if windowed(clusterer):
+    # max_clusters None or >= 32: windows of block Lanczos on the complement of the pairs found,
+    # until the eigengap is decided (as predict() above the dense solver's n).  Every decision is
+    # made on w, which is bitwise the same on every rank.
+    limit = min(n, clusterer.max_clusters + 1) if clusterer.max_clusters else n
+    ops = ShardedOps(*op, width=int(nat.load().sc_eigh_block_size(ew.WINDOW_PAIRS)),
+                     capacity=ew.capacity(n, clusterer.max_clusters, clusterer.min_clusters),
+                     **dist_args)
+    prefix = ew.solve(ops, descend, clusterer.max_clusters, clusterer.min_clusters,
+                      clusterer.stop_eigenvalue, clusterer.eigengap_type, n=n)
+    w = prefix.values[:limit]
+    k, gap = clusterer._count_clusters(w, descend, prefix.lambda_max)
+    columns = min(len(w), max(k, clusterer.min_clusters or 0, 1))
+    v = ops.vectors(prefix.order[:columns])
+    solver, stats = "lanczos-windows-sharded x%d" % world, ops.stats
+  else:
+    limit = min(n, clusterer.max_clusters + 1)
+    n_vectors = min(n, max(limit, clusterer.min_clusters or 0))
+    ops = ShardedOps(*op, width=int(nat.load().sc_eigh_block_size(limit)), **dist_args)
+    w, v, stats = ops.extremal(which, limit, n_vectors)
+    if not descend and clusterer.eigengap_type == utils.EigenGapType.NormalizedDiff:
+      # np.max(eigenvalues) of the full spectrum (utils.py:109): one more extremal solve
+      w = np.concatenate([w, ops.extremal(nat.EIG_LARGEST, 1, 0)[0]])
+    k, gap = clusterer._count_clusters(w, descend)
+    solver, stats = "lanczos-sharded x%d" % world, stats.tolist()
+  clusterer.last_details = dict(eigenvalues=np.array(w[:limit]), n_clusters_raw=k, max_gap=gap,
+                                solver=solver,
                                 transport=getattr(refiner, "last_transport", "local"),
-                                lanczos_stats=stats.tolist())
+                                lanczos_stats=stats)
   return clusterer._cluster_embeddings(eng, v, k)
 
 

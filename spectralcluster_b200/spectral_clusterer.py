@@ -183,9 +183,8 @@ class SpectralClusterer:
       # more pairs than one Lanczos solve finds, above the dense solver's n: windows of block
       # Lanczos on the complement of the pairs found, until the eigengap is decided
       solver, top_solve = "lanczos-windows", None
-      ops = eigen_windows.DeviceOps(eng, *op, which, capacity=min(
-          n, eigen_windows.MAX_WINDOW_PAIRS,
-          max(limit, self.min_clusters or 0) + eigen_windows.WINDOW_PAIRS))
+      ops = eigen_windows.DeviceOps(eng, *op, which, capacity=eigen_windows.capacity(
+          n, self.max_clusters, self.min_clusters))
       prefix = eigen_windows.solve(ops, descend, self.max_clusters, self.min_clusters,
                                    self.stop_eigenvalue, self.eigengap_type, n=n)
       w, top = prefix.values[:limit], prefix.lambda_max
