@@ -239,6 +239,16 @@ int sc_gemm_nt_planes(sc_context* ctx, int precision, const void* a_hi, const vo
                       int64_t n, int64_t k, float* c, int64_t ldc, float* c_mirror, int64_t ldm,
                       void* stream);
 
+/* Row statistics of the single-MMA product a_hi[m,k] b_hi[n,k]^T without storing it: rowmax[i]
+ * (fp32) and rowsum[i] (fp64) for i < m are FOLDED INTO (maximum and sum, not reset; start them at
+ * 0 -- the products are non-negative) so that a row block of S = Y Y^T can be streamed over column
+ * chunks.  a_hi == b_hi with m == n takes the symmetric launch of sc_diffuse (upper tiles, mirrored
+ * column statistics).  fp16 operands: 16-byte aligned bases, lda/ldb % 8 == 0.  The row-sharded
+ * factored route's RowWiseNormalize maxima and Laplacian degrees. */
+int sc_diffuse_stats_block(sc_context* ctx, const void* a_hi, int64_t lda, int64_t m,
+                           const void* b_hi, int64_t ldb, int64_t n, int64_t k, float* rowmax,
+                           double* rowsum, void* stream);
+
 /* ---- constraint operators (constraint.py:95-164) ---------------------------------------------- */
 /* Element-wise: mode 0 max(a, q) (AffinityIntegration Max, :112-113); 1 (a + q)/2 (Average,
  * :114-115); 2 q > 0 ? 1 - (1 - q)(1 - a) : (1 + q) a (the propagation's final adjustment,
@@ -344,6 +354,34 @@ int sc_eigh_extremal_locked_sharded(sc_context* ctx, const float* s_block, int64
                                     double* y_slabs, int slab, int64_t slab_len,
                                     sc_gather_fn gather, void* user, double* w_host,
                                     int64_t* stats_host, void* stream);
+
+/* Row-sharded FACTORED operator: as sc_eigh_extremal_sharded, with S = Y Y^T never formed.
+ * `y_rows` holds rows [row_begin, row_begin+rows) of Y's fp16 hi plane (16-byte aligned, ldy % 8
+ * == 0).  Every pass is two half-products.  First this rank's share of Z = Y^T T, Y[R,:]^T T[R],
+ * is written to y_slabs[0 .. b N) (vector-major, stride N) and gather(user, -b) is called: it must
+ * SUM those b N doubles over the ranks in place, leaving bitwise the same result on every rank (an
+ * all-reduce).  Then Y[R,:] Z is written to this rank's slab and gather(user, b) all-gathers it as
+ * in sc_eigh_extremal_sharded.  Y need not be symmetric. */
+int sc_eigh_extremal_factored_sharded(sc_context* ctx, const void* y_rows, int64_t rows,
+                                      int64_t row_begin, int64_t n, int64_t ldy,
+                                      const double* delta, const double* left, const double* right,
+                                      double sign, int which, int64_t n_values, int64_t n_vectors,
+                                      double tol, int64_t max_matvecs, double* y_slabs, int slab,
+                                      int64_t slab_len, sc_gather_fn gather, void* user,
+                                      double* w_host, double* v_dev, int64_t* stats_host,
+                                      void* stream);
+
+/* One window of a windowed solve on the row-sharded factored operator: the arguments of
+ * sc_eigh_extremal_locked_sharded with `y_rows` / `ldy` in place of `s_block` / `lds`. */
+int sc_eigh_extremal_locked_factored_sharded(sc_context* ctx, const void* y_rows, int64_t rows,
+                                             int64_t row_begin, int64_t n, int64_t ldy,
+                                             const double* delta, const double* left,
+                                             const double* right, double sign, int which,
+                                             int64_t n_values, double tol, int64_t max_matvecs,
+                                             double scale, double* locked, int64_t n_locked,
+                                             double* y_slabs, int slab, int64_t slab_len,
+                                             sc_gather_fn gather, void* user, double* w_host,
+                                             int64_t* stats_host, void* stream);
 
 /* The block product of the extremal solver on its own (the O(N^2) part of what replaces
  * np.linalg.eig at utils.py:59): y[p][0..rows) = s[0..rows, 0..n) t[p][0..n) for p < b <= 16; `s` fp32

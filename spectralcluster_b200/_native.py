@@ -67,6 +67,8 @@ PROTOTYPES = {
     "sc_transpose": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr],
     "sc_gemm_nt_planes": [c_ptr, c_int, c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_i64, c_i64,
                           c_i64, c_ptr, c_i64, c_ptr, c_i64, c_ptr],
+    "sc_diffuse_stats_block": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_i64, c_i64, c_ptr,
+                               c_ptr, c_ptr],
     "sc_constraint_combine": [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_int, c_ptr, c_i64, c_ptr],
     "sc_scale_shift": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_dbl, c_dbl, c_ptr, c_i64, c_ptr],
     "sc_gemm_nt_f32": [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr],
@@ -89,6 +91,13 @@ PROTOTYPES = {
                                         c_ptr, c_dbl, c_int, c_i64, c_dbl, c_i64, c_dbl, c_ptr,
                                         c_i64, c_ptr, c_int, c_i64, c_ptr, c_ptr, c_ptr, c_ptr,
                                         c_ptr],
+    "sc_eigh_extremal_factored_sharded": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr,
+                                          c_ptr, c_dbl, c_int, c_i64, c_i64, c_dbl, c_i64, c_ptr,
+                                          c_int, c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_eigh_extremal_locked_factored_sharded": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr,
+                                                 c_ptr, c_ptr, c_dbl, c_int, c_i64, c_dbl, c_i64,
+                                                 c_dbl, c_ptr, c_i64, c_ptr, c_int, c_i64, c_ptr,
+                                                 c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_block_product": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, ctypes.c_int, c_ptr, c_i64,
                          c_ptr],
     "sc_block_product_f16": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr, c_i64, ctypes.c_int, c_ptr,

@@ -203,6 +203,22 @@ extern "C" int sc_gemm_nt_planes(sc_context* ctx, int precision, const void* a_h
                          as_stream(stream));
 }
 
+// Row statistics of the single-MMA product a_hi[m,k] b_hi[n,k]^T, nothing stored: the epilogue of
+// sc_diffuse(s == NULL) on a rectangular block.  rowmax (fp32) and rowsum (fp64) are indexed by the
+// rows of a and are folded into, not reset, so that a row's statistics accumulate over column
+// blocks.  When a and b are the same rows (a_hi == b_hi, m == n) the symmetric launch computes the
+// upper tiles only and folds the mirrored column statistics, as sc_diffuse does.
+extern "C" int sc_diffuse_stats_block(sc_context* ctx, const void* a_hi, int64_t lda, int64_t m,
+                                      const void* b_hi, int64_t ldb, int64_t n, int64_t k,
+                                      float* rowmax, double* rowsum, void* stream) {
+  SC_REQUIRE(ctx && a_hi && b_hi && rowmax && rowsum && m > 0 && n > 0 && k > 0,
+             "sc_diffuse_stats_block: bad arguments");
+  return gemm_nt_wgmma(ctx, 0, SC_GEMM_SINGLE, (const __half*)a_hi, nullptr, lda,
+                         (const __half*)b_hi, nullptr, ldb, m, n, k, nullptr, 0, nullptr,
+                         /*symmetric=*/true, /*diag_shift=*/0, rowmax, rowsum, nullptr, 0,
+                         as_stream(stream));
+}
+
 // c[m,n] = a[m,k] b[n,k]^T with fp32 operands on the SIMT engine (fp64 accumulation): the small-
 // matrix twin of sc_gemm_nt_planes for the constraint propagation products (constraint.py:147-153).
 extern "C" int sc_gemm_nt_f32(sc_context* ctx, const float* a, int64_t lda, const float* b,

@@ -819,7 +819,6 @@ static int blur_thrsym_rows(const char* who, sc_context* ctx, const float* a, in
                             int preserve_diagonal, int sym_type, float* y, int64_t ldy, void* hi,
                             void* lo, int64_t ldh, void* stream) {
   SC_REQUIRE(ctx && a && rowmax && n > 0, "%s: bad arguments", who);
-  SC_REQUIRE((hi == nullptr) == (lo == nullptr), "hi/lo must come together");
   RuleArgs r;
   if (int rc = rule_args(who, rowmax, p, mult, binarize, preserve_diagonal, sym_type, y, ldy, hi,
                          lo, ldh, r))

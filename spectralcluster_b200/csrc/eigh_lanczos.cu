@@ -280,6 +280,70 @@ __global__ void k_postscale(const double* __restrict__ x, const double* __restri
   w[o] = flip * ((delta ? delta[i] * x[o] : 0.0) + sign * c * y[yi]);
 }
 
+// Transposed block product over local rows: partial[split][p][c] = sum over the rows r of the
+// split of y[r, c] t[p][r] (fp16 -> fp64 exactly, fp64 accumulation in row order).  One thread per
+// column, so a warp reads 64 contiguous bytes of a row; t is read uniformly (a broadcast).
+template <int B>
+__global__ void __launch_bounds__(256)
+k_colprod_f16(const __half* __restrict__ y, int64_t rows, int64_t n, int64_t ldy,
+              const double* __restrict__ t, int64_t ldt, int b, int64_t rows_per_split,
+              double* __restrict__ partial) {
+  const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n) return;
+  const int64_t r0 = (int64_t)blockIdx.y * rows_per_split;
+  const int64_t r1 = min(rows, r0 + rows_per_split);
+  double acc[B];
+#pragma unroll
+  for (int p = 0; p < B; ++p) acc[p] = 0.0;
+  for (int64_t r = r0; r < r1; ++r) {
+    const double v = (double)__half2float(y[r * ldy + c]);
+#pragma unroll
+    for (int p = 0; p < B; ++p)
+      if (p < b) acc[p] = fma(v, t[(int64_t)p * ldt + r], acc[p]);
+  }
+  double* out = partial + (int64_t)blockIdx.y * b * n;
+#pragma unroll
+  for (int p = 0; p < B; ++p)
+    if (p < b) out[(int64_t)p * n + c] = acc[p];
+}
+
+template <int B>
+static void launch_colprod(const __half* y, int64_t rows, int64_t n, int64_t ldy, const double* t,
+                           int64_t ldt, int b, int splits, int64_t rows_per_split, double* partial,
+                           cudaStream_t st) {
+  k_colprod_f16<B><<<dim3((unsigned)((n + 255) / 256), (unsigned)splits), 256, 0, st>>>(
+      y, rows, n, ldy, t, ldt, b, rows_per_split, partial);
+  sc::launched();
+}
+
+// z[p][c] = sum over the splits, in order, of partial[split][p][c] (z: stride n)
+__global__ void k_colprod_reduce(const double* __restrict__ partial, int splits, int b, int64_t n,
+                                 double* __restrict__ z) {
+  const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n) return;
+  const int p = blockIdx.y;
+  double acc = 0.0;
+  for (int sp = 0; sp < splits; ++sp) acc += partial[((int64_t)sp * b + p) * n + c];
+  z[(int64_t)p * n + c] = acc;
+}
+
+// row splits of the transposed block product: enough CTAs to fill the device
+static int colprod_splits(int64_t rows, int64_t n, int sm_count) {
+  const int64_t col_blocks = (n + 255) / 256;
+  int64_t splits = (8LL * sm_count + col_blocks - 1) / col_blocks;
+  const int64_t max_splits = (rows + 255) / 256;           // at least 256 rows per split
+  return (int)std::max<int64_t>(1, std::min(splits, max_splits));
+}
+
+// t[p][i] = y[i / slab_len][p][i % slab_len]: gathered slabs back to vector-major (stride ldt)
+__global__ void k_unslab(const double* __restrict__ y, int64_t slab_len, int nb, int64_t n,
+                         double* __restrict__ t, int64_t ldt) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int p = blockIdx.y;
+  t[(int64_t)p * ldt + i] = y[(i / slab_len) * nb * slab_len + (int64_t)p * slab_len + i % slab_len];
+}
+
 // h[j] = <V_j, w>, one CTA per basis vector (deterministic tree reduction)
 __global__ void k_proj(const double* __restrict__ v, int64_t n, const double* __restrict__ w,
                        double* __restrict__ h) {
@@ -688,7 +752,9 @@ typedef int (*sc_gather_fn)(void* user, int count);
 // and relative to the operator's scale is the accuracy its callers need.
 // Factored operator (sc_eigh_extremal_factored): `s` is NULL and yh = Y (fp16, symmetric) stands
 // for S = Y Y^T; every block product is Y (Y T) through an [b][n] fp64 intermediate, two passes of
-// 2 B per element over Y.
+// 2 B per element over Y.  Row-sharded factored operator (sc_eigh_extremal_factored_sharded): yh
+// holds the local rows of Y; Y^T T is summed over the ranks (gather(user, -b)) and Y (Y^T T) is
+// all-gathered (gather(user, b)): two collectives per pass.
 static int lanczos_impl(sc_context* ctx, const float* s, const __half* yh, int64_t rows,
                         int64_t row_begin,
                         int64_t n, int64_t lds, const double* delta, const double* left,
@@ -699,7 +765,8 @@ static int lanczos_impl(sc_context* ctx, const float* s, const __half* yh, int64
                         double* w_host, double* v_dev, int64_t* stats_host, void* stream) {
   SC_REQUIRE(ctx && (s != nullptr) != (yh != nullptr) && w_host && n > 0,
              "sc_eigh_extremal: bad arguments");
-  SC_REQUIRE(!yh || (rows == n && y_ext == nullptr), "sc_eigh_extremal: internal (factored operator)");
+  SC_REQUIRE(!yh || (rows == n && y_ext == nullptr) || (y_ext && gather),
+             "sc_eigh_extremal: internal (factored operator)");
   SC_REQUIRE(n_values >= 1 && n_values <= 32 && n_vectors >= 0 && n_vectors <= n_values,
              "sc_eigh_extremal: need 1 <= n_values <= 32 and n_vectors <= n_values");
   SC_REQUIRE(n_vectors == 0 || v_dev, "sc_eigh_extremal: v_dev missing");
@@ -844,6 +911,11 @@ static int lanczos_impl(sc_context* ctx, const float* s, const __half* yh, int64
   Scratch prod_buf;
   SC_CUDA(prod_buf.alloc(sizeof(double) * block_product_scratch_doubles(rows, n, b, ctx->sm_count,
                                                                         &prod_splits, &prod_cols), st));
+  // transposed block product of the row-sharded factored operator
+  const int colp_splits = (yh && y_ext) ? colprod_splits(rows, n, ctx->sm_count) : 0;
+  const int64_t colp_rows = colp_splits ? (rows + colp_splits - 1) / colp_splits : 0;
+  Scratch colp_buf;
+  if (colp_splits) SC_CUDA(colp_buf.alloc(sizeof(double) * (size_t)colp_splits * b * n, st));
   int P = 0, J = b;
   int64_t matvecs = 0, restarts = 0, passes = 0;
   int converged = 0, mm = 0;
@@ -891,7 +963,20 @@ static int lanczos_impl(sc_context* ctx, const float* s, const __half* yh, int64
   for (;;) {
     // ---- one pass over S: W = flip * Op V[P..P+b)
     k_prescale<<<dim3(gn, b), 256, 0, st>>>(V + (size_t)P * n, left, right, n, tb, ldtb); sc::launched();
-    if (yh) {
+    if (yh && y_ext) {
+      // row-sharded factored operator: this rank's share of Z = Y^T T, Y[R,:]^T T[R], into
+      // y_ext[0 .. b n) (vector-major, stride n), summed over the ranks by gather(user, -b) and
+      // copied into `mid`; then Y[R,:] Z, row block R of Y Y^T T.  No symmetry of Y is assumed.
+      SC_BLOCK_DISPATCH(b, launch_colprod<B_>(yh, rows, n, lds, tb + row_begin, ldtb, b, colp_splits,
+                                                colp_rows, colp_buf.as<double>(), st));
+      k_colprod_reduce<<<dim3(gn, b), 256, 0, st>>>(colp_buf.as<double>(), colp_splits, b, n, y_ext);
+      sc::launched();
+      SC_LAUNCH_CHECK();
+      SC_REQUIRE(gather(user, -b) == 0, "sc_eigh_extremal_sharded: the gather callback failed");
+      k_unslab<<<dim3(gn, b), 256, 0, st>>>(y_ext, n, b, n, mid, ldtb); sc::launched();
+      if (int rc = launch_block_product(b, yh, rows, n, lds, mid, ldtb, y_mine, y_slab_len,
+                                        prod_buf.as<double>(), prod_splits, prod_cols, st)) return rc;
+    } else if (yh) {
       if (int rc = launch_block_product(b, yh, rows, n, lds, tb, ldtb, mid, ldtb,
                                         prod_buf.as<double>(), prod_splits, prod_cols, st)) return rc;
       if (int rc = launch_block_product(b, yh, rows, n, lds, mid, ldtb, y_mine, y_slab_len,
@@ -1167,6 +1252,45 @@ extern "C" int sc_eigh_extremal_locked_sharded(sc_context* ctx, const float* s_b
   return lanczos_impl(ctx, s_block, nullptr, rows, row_begin, n, lds, delta, left, right, sign, which,
                       n_values, 0, tol, max_matvecs, y_slabs, slab, slab_len, gather, user, locked,
                       n_locked, scale, w_host, nullptr, stats_host, stream);
+}
+
+// Row-sharded factored operator: `y_rows` holds rows [row_begin, row_begin+rows) of Y (fp16 hi
+// plane) and S = Y Y^T is never formed.  Every pass over the operator is two half-products:
+// Y[R,:]^T T[R], summed over the ranks by gather(user, -b), and Y[R,:] Z, all-gathered by
+// gather(user, b).
+extern "C" int sc_eigh_extremal_factored_sharded(sc_context* ctx, const void* y_rows, int64_t rows,
+                                                 int64_t row_begin, int64_t n, int64_t ldy,
+                                                 const double* delta, const double* left,
+                                                 const double* right, double sign, int which,
+                                                 int64_t n_values, int64_t n_vectors, double tol,
+                                                 int64_t max_matvecs, double* y_slabs, int slab,
+                                                 int64_t slab_len, sc_gather_fn gather, void* user,
+                                                 double* w_host, double* v_dev, int64_t* stats_host,
+                                                 void* stream) {
+  SC_REQUIRE(y_rows && y_slabs && gather && rows > 0 && row_begin >= 0 && row_begin + rows <= n,
+             "sc_eigh_extremal_factored_sharded: bad arguments");
+  SC_REQUIRE(slab >= 0 && slab_len > 0 && row_begin == (int64_t)slab * slab_len && rows <= slab_len,
+             "sc_eigh_extremal_factored_sharded: rank `slab` must own rows [slab*slab_len, +rows)");
+  return lanczos_impl(ctx, nullptr, (const __half*)y_rows, rows, row_begin, n, ldy, delta, left,
+                      right, sign, which, n_values, n_vectors, tol, max_matvecs, y_slabs, slab,
+                      slab_len, gather, user, nullptr, 0, 0.0, w_host, v_dev, stats_host, stream);
+}
+
+// One window of the windowed solve on the row-sharded factored operator (locked set replicated).
+extern "C" int sc_eigh_extremal_locked_factored_sharded(
+    sc_context* ctx, const void* y_rows, int64_t rows, int64_t row_begin, int64_t n, int64_t ldy,
+    const double* delta, const double* left, const double* right, double sign, int which,
+    int64_t n_values, double tol, int64_t max_matvecs, double scale, double* locked,
+    int64_t n_locked, double* y_slabs, int slab, int64_t slab_len, sc_gather_fn gather, void* user,
+    double* w_host, int64_t* stats_host, void* stream) {
+  SC_REQUIRE(y_rows && y_slabs && gather && locked && rows > 0 && row_begin >= 0 &&
+             row_begin + rows <= n, "sc_eigh_extremal_locked_factored_sharded: bad arguments");
+  SC_REQUIRE(slab >= 0 && slab_len > 0 && row_begin == (int64_t)slab * slab_len && rows <= slab_len,
+             "sc_eigh_extremal_locked_factored_sharded: rank `slab` must own rows "
+             "[slab*slab_len, +rows)");
+  return lanczos_impl(ctx, nullptr, (const __half*)y_rows, rows, row_begin, n, ldy, delta, left,
+                      right, sign, which, n_values, 0, tol, max_matvecs, y_slabs, slab, slab_len,
+                      gather, user, locked, n_locked, scale, w_host, nullptr, stats_host, stream);
 }
 
 // ---------------------------------------------------------------------------------------------

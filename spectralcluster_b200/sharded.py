@@ -19,6 +19,11 @@ row block [row_begin, row_end) of every N x N matrix:
      tests, boxes without IPC) moves the same blocks with batched send/recv instead;
   6. row maxima / sums of S_block (RowWiseNormalize, Laplacian degree) are row-local.
 
+Above the size where those per-rank buffers fit (sharded_stored_peak_bytes), the factored route
+(FactoredShardedRefiner) keeps only the owned rows of Y's fp16 hi plane and never stores S: the
+front end runs in row panels, S's row statistics are streamed over chunks of the peers' Y rows,
+and the eigensolver applies S = Y Y^T as two half-products per pass.
+
 The orchestration below is backend-agnostic: `DeviceBackend` runs the CUDA kernels through the C
 ABI; the CPU tests plug in a NumPy backend and run the same code under gloo with 2 ranks.
 """
@@ -34,6 +39,62 @@ import numpy as np
 
 def _round_up(x: int, m: int) -> int:
   return (x + m - 1) // m * m
+
+
+# The factored route streams the peers' Y rows through two staging buffers of about this many
+# bytes each: a fixed size, whatever N and the world size.
+STAGING_BYTES = 1 << 28
+
+
+def sharded_stored_peak_bytes(n: int, world: int) -> int:
+  """Per-rank device bytes of the stored sharded route's N x N-scale buffers, computed from shapes:
+  both fp16 planes of Y at full size (world * block rows) and the fp32 arena that holds the halo'd
+  affinity block and then S's row block (block + blur halo + 2 x 64 rows)."""
+  from .device import BLUR_HALO, round_up
+  block = _round_up(int(math.ceil(n / world)), 128)
+  ld = round_up(n, 64)
+  return 4 * world * block * ld + 4 * (block + 2 * BLUR_HALO + 2 * 64) * ld
+
+
+def sharded_factored_peak_bytes(n: int, world: int) -> int:
+  """Per-rank device bytes of the factored sharded route's large buffers, computed from shapes:
+  the owned rows of Y_hi (fp16), one fp32 affinity panel with its halo, and the two staging
+  buffers.  Nothing in it is N x N."""
+  from .device import panel_rows_for, round_up
+  block = _round_up(int(math.ceil(n / world)), 128)
+  ld = round_up(n, 64)
+  panel = min(panel_rows_for(n), block)
+  staging = 2 * 2 * staging_rows_for(n) * ld if world > 1 else 0
+  return 2 * block * ld + 4 * (panel + 2 * 64) * ld + staging
+
+
+def staging_rows_for(n: int) -> int:
+  """Rows of peer Y_hi per staging buffer: about STAGING_BYTES of fp16 rows, a multiple of 128."""
+  from .device import round_up
+  return max(128, STAGING_BYTES // (2 * round_up(n, 64)) // 128 * 128)
+
+
+def factored_sharded_route(eng, n: int, world: int) -> bool:
+  """Whether predict_sharded() takes the factored route: the stored sharded route's per-rank peak
+  (computed from shapes) exceeds eng.factored_above_bytes, and Diffuse is the single-MMA product
+  whose operand is Y's hi plane alone.  Decided from n, the world size, the options and the
+  device's total memory, never from what is free, as predict()'s own route choice."""
+  from . import _native as nat
+  return (sharded_stored_peak_bytes(n, world) > eng.factored_above_bytes and
+          eng.diffuse_precision_for(n) == nat.GEMM_SINGLE)
+
+
+class RowPanel(typing.NamedTuple):
+  """Output rows [row_begin, row_end) of one front-end panel, computed from the affinity rows
+  [halo_begin, halo_end) (the blur halo clipped at 0 and n)."""
+  row_begin: int
+  row_end: int
+  halo_begin: int
+  halo_end: int
+
+  @property
+  def halo_rows(self) -> int:
+    return self.halo_end - self.halo_begin
 
 
 class ShardPlan:
@@ -295,6 +356,103 @@ class ShardedRefiner:
     self.dist.all_gather_into_tensor(full, mine, group=self.group)
 
 
+class FactoredShardedRefiner(ShardedRefiner):
+  """The refinement of ShardedRefiner with S never stored and Y kept for the owned rows only.
+
+  1. front end in row panels of the owned rows (two passes, as device.FactoredAffinity): pass 1
+     computes each panel's affinity rows plus the blur halo and folds the blur row maxima into m,
+     which is all-gathered (N floats); pass 2 recomputes the panel's affinity and writes its rows
+     of Y's fp16 hi plane (no lo plane) into a rows x ld buffer;
+  2. S's row maxima and sums of the owned rows: the own block by the symmetric statistics-only
+     GEMM, then every peer's Y rows in chunks through two fixed-size staging buffers (send/recv),
+     each chunk's statistics folded by the statistics-only GEMM.  S(g, :) is computed in full
+     by every rank: twice the flops of the stored route's symmetric split.
+  run() returns the owned Y_hi rows with the row maxima / sums."""
+
+  def __init__(self, backend, options, dist=None, group=None, panel_rows=None):
+    super().__init__(backend, options, dist=dist, group=group)
+    self.panel_rows = panel_rows
+
+  def panels(self, plan):
+    from .device import panel_rows_for
+    step = self.panel_rows or panel_rows_for(plan.n)
+    out = []
+    for r0 in range(plan.row_begin, plan.row_end, step):
+      r1 = min(plan.row_end, r0 + step)
+      out.append(RowPanel(r0, r1, max(0, r0 - plan.radius), min(plan.n, r1 + plan.radius)))
+    return out
+
+  def run(self, embeddings, world: int = 1, rank: int = 0):
+    from .device import blur_radius
+    be, opt = self.backend, self.options
+    n = int(embeddings.shape[0])
+    plan = ShardPlan(n, world, rank, blur_radius(self.sigma))
+    panels = self.panels(plan)
+    capacity = max(p.halo_rows for p in panels)
+    zero_diag = bool(opt.thresholding_preserve_diagonal)
+    self._mark("start")
+    planes = be.normalize(embeddings)
+    m_full = be.new_row_vector(world * plan.block)
+    for p in panels:
+      a, crop = be.affinity_block(planes, n, p.halo_begin, p.halo_rows, self.has_crop, capacity)
+      be.blur_rowmax_block(a, n, p, crop, self.sigma, zero_diag, m_full)
+    if world > 1:
+      self._all_gather_blocks(m_full, plan)
+    self._mark("rowmax gathered")
+    y_rows = be.new_rows(plan.rows, n)
+    for p in panels:
+      a, crop = be.affinity_block(planes, n, p.halo_begin, p.halo_rows, self.has_crop, capacity)
+      be.thrsym_rows(a, n, p, crop, self.sigma, m_full, opt, self.sym_max, y_rows, None,
+                     plan.row_begin)
+    del a
+    self._mark("Y rows done")
+    rowmax, rowsum = self._row_stats(plan, y_rows, n)
+    self._mark("row stats")
+    return dict(plan=plan, y_rows=y_rows, rowmax=rowmax, rowsum=rowsum)
+
+  def _row_stats(self, plan, y_rows, n):
+    """Row maxima and sums of S(g, :) = Y[R_g] Y^T, S never stored."""
+    be, world, rank = self.backend, plan.world, plan.rank
+    mx, sm = be.new_stats(plan.rows)
+    be.stats_block(y_rows, plan.rows, y_rows, plan.rows, n, mx, sm)     # own block, symmetric
+    self.last_transport = self.dist.get_backend(self.group) if world > 1 else "local"
+    if world == 1:
+      return mx, sm
+    staging, chunk = be.staging(n)
+    be.reserve_comm_sms(True)        # leave SMs to the send/recv kernels during the GEMMs
+    try:
+      for o in range(1, world):
+        # step o: receive the rows of rank + o, send mine to rank - o (every pair matches)
+        src, dst = (rank + o) % world, (rank - o) % world
+        lo, hi = plan.rows_of(src)
+        recv = [(c0, min(c0 + chunk, hi - lo)) for c0 in range(0, hi - lo, chunk)]
+        send = [(c0, min(c0 + chunk, plan.rows)) for c0 in range(0, plan.rows, chunk)]
+
+        def post(j):
+          sends = [(y_rows[send[j][0]:send[j][1]], dst)] if j < len(send) else []
+          recvs = ([(staging[j % 2][:recv[j][1] - recv[j][0]], src)] if j < len(recv) else [])
+          return self._p2p(sends, recvs)
+
+        steps = max(len(recv), len(send))
+        pending, works = post(0), []
+        for j in range(steps):
+          recv_w, all_w = pending
+          works += all_w
+          # chunk j + 1 lands in the other buffer while chunk j is multiplied; the GEMM of chunk
+          # j - 1, which read that buffer, is already ordered before it on the stream
+          pending = post(j + 1) if j + 1 < steps else ([], [])
+          for w in recv_w:
+            w.wait()
+          if j < len(recv):
+            c0, c1 = recv[j]
+            be.stats_block(y_rows, plan.rows, staging[j % 2], c1 - c0, n, mx, sm)
+        for w in works:
+          w.wait()
+    finally:
+      be.reserve_comm_sms(False)
+    return mx, sm
+
+
 class DeviceBackend:
   """The CUDA kernels behind the C ABI (wgmma GEMMs, fused blur passes)."""
 
@@ -331,12 +489,14 @@ class DeviceBackend:
              x.stride(0), None, 0, self._p(hi), self._p(lo), hi.stride(0), eng.stream)
     return hi, lo, d
 
-  def affinity_block(self, planes, n, row_begin, row_count, want_crop):
+  def affinity_block(self, planes, n, row_begin, row_count, want_crop, capacity=None):
+    """Affinity rows [row_begin, +row_count) in the arena; `capacity` (rows) keeps one arena for
+    panels of different heights."""
     eng, t = self.eng, self.t
     hi, lo, d = planes
     ld = self.dev.round_up(n, 64)
     # the halo'd affinity block is dead before S_block is written: both live in one arena
-    arena = self._buffer("arena", (max(row_count, 1) + 2 * 64, ld), t.float32)
+    arena = self._buffer("arena", (max(row_count, capacity or 0, 1) + 2 * 64, ld), t.float32)
     a = arena[:row_count]
     crop = t.zeros((n,), dtype=t.float32, device=eng.device) if want_crop else None
     eng.call("sc_affinity_cosine_block", eng.gemm_precision, self._p(hi), self._p(lo),
@@ -367,17 +527,49 @@ class DeviceBackend:
              float(sigma), int(zero_diag), self._p(m_full), eng.stream)
 
   def thrsym_block(self, a_ext, n, plan, crop, sigma, m_full, opt, sym_max, y_full):
+    self.thrsym_rows(a_ext, n, plan, crop, sigma, m_full, opt, sym_max, y_full[0], y_full[1], 0)
+
+  def thrsym_rows(self, a_ext, n, rows, crop, sigma, m_full, opt, sym_max, hi, lo, first_row):
+    """Y rows [rows.row_begin, rows.row_end) into planes whose row 0 is global row first_row
+    (`lo` None: the hi plane only)."""
     eng, nat = self.eng, self.nat
-    hi, lo = y_full
-    off = plan.row_begin * hi.stride(0) * 2
+    off = (rows.row_begin - first_row) * hi.stride(0) * 2
     c = self.dev.ctypes.c_void_p
     eng.call("sc_blur_threshold_symmetrize_block", self._p(a_ext), n, a_ext.stride(0),
-             plan.halo_begin, plan.halo_rows, plan.row_begin, plan.row_end, self._p(crop),
+             rows.halo_begin, rows.halo_rows, rows.row_begin, rows.row_end, self._p(crop),
              float(sigma), self._p(m_full), float(opt.p_percentile),
              float(opt.thresholding_soft_multiplier), int(bool(opt.thresholding_with_binarization)),
              int(bool(opt.thresholding_preserve_diagonal)),
              nat.SYMMETRIZE_MAX if sym_max else nat.SYMMETRIZE_AVERAGE, None, 0,
-             c(hi.data_ptr() + off), c(lo.data_ptr() + off), hi.stride(0), eng.stream)
+             c(hi.data_ptr() + off), None if lo is None else c(lo.data_ptr() + off), hi.stride(0),
+             eng.stream)
+
+  # ---- factored route: owned Y_hi rows, S's row statistics streamed
+  def new_rows(self, rows, n):
+    """The owned rows of Y's hi plane.  The stored route's full-size planes are released first:
+    the two routes never run on the same call."""
+    self.release("y_hi", "y_lo")
+    return self._buffer("y_rows", (rows, self.dev.round_up(n, 64)), self.t.float16)
+
+  def release(self, *tags):
+    for k in [k for k in self._buffers if k[0] in tags]:
+      del self._buffers[k]
+
+  def new_stats(self, rows):
+    t = self.t
+    return (t.zeros((rows,), dtype=t.float32, device=self.eng.device),
+            t.zeros((rows,), dtype=t.float64, device=self.eng.device))
+
+  def stats_block(self, a, a_rows, b, b_rows, n, mx, sm):
+    """mx / sm (rows of a) <- max / + the row maxima / sums of a[:a_rows] b[:b_rows]^T (K = n)."""
+    self.eng.call("sc_diffuse_stats_block", self._p(a), a.stride(0), a_rows, self._p(b),
+                  b.stride(0), b_rows, n, self._p(mx), self._p(sm), self.eng.stream)
+
+  def staging(self, n):
+    """Two staging buffers for peer Y_hi rows, and their height in rows."""
+    rows = staging_rows_for(n)
+    buf = self._buffer("staging", (2, rows, self.dev.round_up(n, 64)), self.t.float16)
+    return [buf[0], buf[1]], rows
 
   def gemm_block(self, y_full, a_row, a_rows, b_row, b_rows, n, s_block, s_row, mirror=None,
                  ldm=0):
@@ -530,7 +722,8 @@ class DeviceBackend:
 
 class ShardedOps:
   """The eigensolver on a row-sharded S: the operator diag(delta) + sign * diag(left) S diag(right)
-  with this rank's row block of S.  Every block product streams the local rows and all-gathers the
+  with this rank's row block of S (factored: its rows of Y_hi, S = Y Y^T applied as Y (Y^T T):
+  Y^T T summed over the ranks, then Y T' all-gathered).  Every block product streams the local rows and all-gathers the
   slabs (b N doubles per pass over S); everything else -- Gram-Schmidt, the locked set, the Ritz
   pairs -- runs replicated on full-length vectors, so every rank returns bitwise identical values.
 
@@ -539,13 +732,17 @@ class ShardedOps:
   `capacity` full-length vectors is replicated on every rank."""
 
   def __init__(self, eng, s_block, plan, n, delta, left, right, sign, which, width: int,
-               dist=None, group=None, capacity: int = 0):
+               dist=None, group=None, capacity: int = 0, factored: bool = False):
     from . import _native as nat
     from . import device as dev
     t = dev.torch()
     self.eng, self.nat, self.ptr = eng, nat, dev._ptr
     self.s_block, self.plan, self.n = s_block, plan, n
     self.delta, self.left, self.right, self.sign, self.which = delta, left, right, sign, which
+    # factored: s_block is this rank's rows of Y_hi (fp16) and S = Y Y^T is never formed
+    self.entry = "sc_eigh_extremal_factored_sharded" if factored else "sc_eigh_extremal_sharded"
+    self.window_entry = ("sc_eigh_extremal_locked_factored_sharded" if factored
+                         else "sc_eigh_extremal_locked_sharded")
     world, rank = plan.world, plan.rank
     # block products land in slabs [rank][vector][block]: one all-gather of contiguous slabs per
     # pass over S completes all `width` (or fewer) vectors on every rank
@@ -553,7 +750,10 @@ class ShardedOps:
 
     def gather(_user, count):
       try:
-        if world > 1:
+        if world > 1 and count < 0:
+          # factored operator: sum this rank's share of Y^T T (-count vectors of length n)
+          dist.all_reduce(y_slabs[:-count * n], group=group)
+        elif world > 1:
           per = count * plan.block
           dist.all_gather_into_tensor(y_slabs[:world * per], y_slabs[rank * per:(rank + 1) * per].clone(),
                                       group=group)
@@ -578,7 +778,7 @@ class ShardedOps:
     w = np.empty(n_values, dtype=np.float64)
     v = t.empty((self.n, n_vectors), dtype=t.float64, device=self.eng.device)
     stats = np.zeros(4, dtype=np.int64)
-    self.eng.call("sc_eigh_extremal_sharded", ptr(s), plan.rows, plan.row_begin, self.n,
+    self.eng.call(self.entry, ptr(s), plan.rows, plan.row_begin, self.n,
                   s.stride(0), ptr(self.delta), ptr(self.left), ptr(self.right), float(self.sign),
                   int(which), n_values, n_vectors, 1e-9, 0, *self._slab_args(),
                   w.ctypes.data_as(ctypes.c_void_p), ptr(v) if n_vectors else None,
@@ -590,7 +790,7 @@ class ShardedOps:
     assert self.count + count <= self.locked.shape[0]
     w = np.empty(count, dtype=np.float64)
     st = np.zeros(4, dtype=np.int64)
-    self.eng.call("sc_eigh_extremal_locked_sharded", ptr(s), plan.rows, plan.row_begin, self.n,
+    self.eng.call(self.window_entry, ptr(s), plan.rows, plan.row_begin, self.n,
                   s.stride(0), ptr(self.delta), ptr(self.left), ptr(self.right), float(self.sign),
                   int(self.which), count, 1e-9, 0, float(self.scale), ptr(self.locked), self.count,
                   *self._slab_args(), w.ctypes.data_as(ctypes.c_void_p),
@@ -663,7 +863,8 @@ def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
   embeddings (a host ndarray, or a float32/float64 tensor already on this rank's GPU) and
   receives the same labels.
 
-  Refinement as in ShardedRefiner; row maxima / sums all-gathered (2 N doubles); eigensolve by the
+  Refinement as in ShardedRefiner, or FactoredShardedRefiner when factored_sharded_route() says
+  the stored route's per-rank buffers do not fit; row maxima / sums all-gathered (2 N doubles); eigensolve by the
   sharded thick-restart Lanczos (each matvec streams the local row block and all-gathers N
   doubles), in windows with a replicated locked set when max_clusters is None or >= 32; eigengap
   and k-means replicated on the [N, k] eigenvectors."""
@@ -693,7 +894,10 @@ def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
     x_dev = t.from_numpy(x).to(eng.device, non_blocking=True)
   n = int(x_dev.shape[0])
   opt = clusterer.refinement_options
-  refiner = ShardedRefiner(be, opt, dist=dist if world > 1 else None, group=group)
+  # the stored route's per-rank buffers do not fit: keep only the owned rows of Y_hi
+  factored = factored_sharded_route(eng, n, world)
+  refiner = (FactoredShardedRefiner if factored else ShardedRefiner)(
+      be, opt, dist=dist if world > 1 else None, group=group)
   res = refiner.run(x_dev, world, rank)
   plan = res["plan"]
   length = world * plan.block
@@ -711,8 +915,10 @@ def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
   r = (1.0 / rowmax) if normalized else None
   delta, left, right, sign, which = lap.terms_from_row_sums(rowsum, r, clusterer.laplacian_type)
   descend = which == nat.EIG_LARGEST
-  op = (eng, res["s_block"], plan, n, delta, left, right, sign, which)
-  dist_args = dict(dist=dist if world > 1 else None, group=group)
+  op = (eng, res["y_rows"] if factored else res["s_block"], plan, n, delta, left, right, sign,
+        which)
+  dist_args = dict(dist=dist if world > 1 else None, group=group, factored=factored)
+  route = "factored-sharded" if factored else "sharded"
   if windowed(clusterer):
     # max_clusters None or >= 32: windows of block Lanczos on the complement of the pairs found,
     # until the eigengap is decided (as predict() above the dense solver's n).  Every decision is
@@ -727,7 +933,7 @@ def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
     k, gap = clusterer._count_clusters(w, descend, prefix.lambda_max)
     columns = min(len(w), max(k, clusterer.min_clusters or 0, 1))
     v = ops.vectors(prefix.order[:columns])
-    solver, stats = "lanczos-windows-sharded x%d" % world, ops.stats
+    solver, stats = "lanczos-windows-%s x%d" % (route, world), ops.stats
   else:
     limit = min(n, clusterer.max_clusters + 1)
     n_vectors = min(n, max(limit, clusterer.min_clusters or 0))
@@ -737,7 +943,7 @@ def predict_sharded(clusterer, embeddings, dist=None, group=None) -> np.ndarray:
       # np.max(eigenvalues) of the full spectrum (utils.py:109): one more extremal solve
       w = np.concatenate([w, ops.extremal(nat.EIG_LARGEST, 1, 0)[0]])
     k, gap = clusterer._count_clusters(w, descend)
-    solver, stats = "lanczos-sharded x%d" % world, stats.tolist()
+    solver, stats = "lanczos-%s x%d" % (route, world), stats.tolist()
   clusterer.last_details = dict(eigenvalues=np.array(w[:limit]), n_clusters_raw=k, max_gap=gap,
                                 solver=solver,
                                 transport=getattr(refiner, "last_transport", "local"),
