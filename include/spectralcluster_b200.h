@@ -154,6 +154,31 @@ int sc_diffuse(sc_context* ctx, int engine, int precision, const float* y, int64
                const void* hi, const void* lo, int64_t ldh, int64_t n, float* s, int64_t lds,
                float* rowmax, double* rowsum, void* stream);
 
+/* ---- bounded Diffuse (DESIGN.md section 5): the row maxima of S = Y Y^T, Y >= 0 and bitwise
+ * symmetric, from only the tiles that can hold one.
+ * sc_row_group_bounds: one pass over the fp16 plane y_hi [n, ldy]: norms[i * groups + g] = |y_i^g|
+ * over the 256-column groups g < groups = ceil(n / 256) (fp32, rounded up), diag_lb[i] <= |y_i|^2
+ * (fp64, rounded down) and rowsum[i] = sum_j y_ij (fp64).
+ * sc_gather_rows_f16: dst row r = src row perm[r], `cols` fp16 elements (cols % 8 == 0).
+ * sc_diffuse_tile_list: the tiles (128 x 192, those the symmetric sc_diffuse launch enumerates) of
+ * the product of the permuted rows Y[perm] whose bound from norms and diag_lb (both indexed by the
+ * original row) does not rule out a row maximum, packed m << 16 | n in the launch's rasterised
+ * order into tiles (room for ceil(n/128) * ceil(n/192) entries); *count (device) receives their
+ * number and *total (device) the number of tiles the full launch computes.  n <= 2^20.
+ * sc_diffuse_rowmax_tiles: rowmax[perm[r]] = max over the listed tiles of row r of Y[perm] Y[perm]^T,
+ * yp_hi = the gathered Y[perm]; every element is the statistics-only sc_diffuse(SC_GEMM_SINGLE)
+ * element bit for bit, so rowmax equals its row maxima.  No host synchronisation. */
+int sc_row_group_bounds(sc_context* ctx, const void* y_hi, int64_t n, int64_t ldy, float* norms,
+                        int64_t groups, double* diag_lb, double* rowsum, void* stream);
+int sc_gather_rows_f16(sc_context* ctx, const void* src, int64_t lds, const int* perm, int64_t rows,
+                       int64_t cols, void* dst, int64_t ldd, void* stream);
+int sc_diffuse_tile_list(sc_context* ctx, const float* norms, int64_t groups, const double* diag_lb,
+                         const int* perm, int64_t n, uint32_t* tiles, int* count, int* total,
+                         void* stream);
+int sc_diffuse_rowmax_tiles(sc_context* ctx, const void* yp_hi, int64_t ldh, int64_t n,
+                            const uint32_t* tiles, const int* count, const int* perm,
+                            float* rowmax, void* stream);
+
 /* Row maxima and row sums (fp64) of an fp32 matrix: the reductions of
  * RowWiseNormalize (refinement.py:243) and of the degree (laplacian.py:41). */
 int sc_row_stats(sc_context* ctx, const float* a, int64_t n, int64_t lda, double* rowmax,

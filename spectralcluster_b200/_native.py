@@ -52,6 +52,10 @@ PROTOTYPES = {
     "sc_split_planes": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_i64, c_ptr],
     "sc_diffuse": [c_ptr, c_int, c_int, c_ptr, c_i64, c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64,
                    c_ptr, c_ptr, c_ptr],
+    "sc_row_group_bounds": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr, c_ptr, c_ptr],
+    "sc_gather_rows_f16": [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr],
+    "sc_diffuse_tile_list": [c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_diffuse_rowmax_tiles": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_row_stats": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     "sc_affinity_stats": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr],
     "sc_row_normalize": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr],

@@ -31,6 +31,11 @@ int gemm_nt_wgmma(const sc_context* ctx, int epi, int precision, const __half* a
                   int64_t ldb, int64_t M, int64_t N, int64_t K, float* C, int64_t ldc,
                   float* rowmax_offdiag, bool symmetric, int diag_shift, float* stat_rowmax,
                   double* stat_rowsum, float* mirror, int64_t ldm, cudaStream_t st);
+int diffuse_tile_list(const float* norms, int G, const double* diag_lb, const int* perm,
+                      int64_t n, uint32_t* list, int* count, int* total, cudaStream_t st);
+int diffuse_rowmax_tiles(const sc_context* ctx, const __half* y_hi, int64_t ldh, int64_t n,
+                         const uint32_t* list, const int* count, const int* row_map,
+                         float* rowmax, cudaStream_t st);
 // rowops.cu
 int crop_diagonal_rows(const float* a, int64_t n, int64_t lda, int64_t row_begin, int64_t rows,
                        float* diag_out, cudaStream_t st);
@@ -137,6 +142,25 @@ extern "C" int sc_diffuse(sc_context* ctx, int engine, int precision, const floa
                          (const __half*)hi, (const __half*)lo, ldh, n, n, n, s, lds, nullptr,
                          /*symmetric=*/true, /*diag_shift=*/0, rowmax, rowsum, nullptr, 0,
                          as_stream(stream));
+}
+
+// ---- bounded Diffuse: row maxima of S = Y Y^T from the tiles that can hold one ----------------
+extern "C" int sc_diffuse_tile_list(sc_context* ctx, const float* norms, int64_t groups,
+                                    const double* diag_lb, const int* perm, int64_t n,
+                                    uint32_t* tiles, int* count, int* total, void* stream) {
+  SC_REQUIRE(ctx && norms && diag_lb && perm && tiles && count && total && n > 0,
+             "sc_diffuse_tile_list: bad arguments");
+  return diffuse_tile_list(norms, (int)groups, diag_lb, perm, n, tiles, count, total,
+                           as_stream(stream));
+}
+
+extern "C" int sc_diffuse_rowmax_tiles(sc_context* ctx, const void* yp_hi, int64_t ldh, int64_t n,
+                                       const uint32_t* tiles, const int* count, const int* perm,
+                                       float* rowmax, void* stream) {
+  SC_REQUIRE(ctx && yp_hi && tiles && count && perm && rowmax && n > 0,
+             "sc_diffuse_rowmax_tiles: bad arguments");
+  return diffuse_rowmax_tiles(ctx, (const __half*)yp_hi, ldh, n, tiles, count, perm, rowmax,
+                              as_stream(stream));
 }
 
 // ---- row-block / general variants used by the row-sharded multi-GPU pipeline ----------------

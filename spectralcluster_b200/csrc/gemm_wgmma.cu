@@ -260,6 +260,11 @@ struct TileCursor {
   }
 };
 
+__device__ __forceinline__ TileCoord listed_tile(const uint32_t* __restrict__ list, int tile) {
+  const uint32_t v = __ldg(list + tile);
+  return TileCoord{(int)(v >> 16), (int)(v & 0xFFFFu)};
+}
+
 template <int PREC, int BN>
 struct StageGeom {
   // planes of one K block in a stage: [A_hi][B_hi][A_lo (PREC>=2)][B_lo (PREC==3)], each a
@@ -271,7 +276,7 @@ struct StageGeom {
   static constexpr int STAGES = (BUDGET / BYTES) > 8 ? 8 : (BUDGET / BYTES);
 };
 
-template <int PREC, int EPI, bool SYM, int BN>
+template <int PREC, int EPI, bool SYM, int BN, bool LIST = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
              const __grid_constant__ CUtensorMap map_a_lo,
@@ -281,7 +286,9 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
              float* __restrict__ C, int64_t ldc, float* __restrict__ rowmax_offdiag,
              int diag_shift, unsigned int* __restrict__ pace, int pace_kb,
              float* __restrict__ stat_rowmax, double* __restrict__ stat_rowsum,
-             float* __restrict__ mirror_out, int64_t ldm, int aff_chunk_kb) {
+             float* __restrict__ mirror_out, int64_t ldm, int aff_chunk_kb,
+             const uint32_t* __restrict__ tile_list, const int* __restrict__ tile_count,
+             const int* __restrict__ row_map) {
   constexpr int STAGES = StageGeom<PREC, BN>::STAGES;
   constexpr int STAGE_BYTES = StageGeom<PREC, BN>::BYTES;
   constexpr int B_PLANE_BYTES = StageGeom<PREC, BN>::B_PLANE_BYTES;
@@ -302,7 +309,10 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
-  const int num_tiles = SYM ? tab.num_tiles : tiles_m * tiles_n;
+  // LIST: the tiles come from a device list (tile_list[0, *tile_count), packed m_blk << 16 | n_blk,
+  // in the rasterised order), row statistics are maxima only, stored through row_map
+  static_assert(!LIST || (SYM && EPI == TC_EPI_PLAIN), "a tile list serves the symmetric Diffuse");
+  const int num_tiles = LIST ? *tile_count : SYM ? tab.num_tiles : tiles_m * tiles_n;
   const int num_kb = (K + BK - 1) / BK;
 
   if (warp == 0 && lane == 0) {
@@ -342,7 +352,7 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
           if (pace) atomicAdd(pace, (unsigned int)ck_per_tile);
           continue;
         }
-        const TileCoord tc = cursor.at(tile, tab);
+        const TileCoord tc = LIST ? listed_tile(tile_list, tile) : cursor.at(tile, tab);
         const int row_a = tc.m_blk * BM, row_b = tc.n_blk * BN;
         for (int kb = 0; kb < num_kb; ++kb) {
           if (pace && kb % pace_kb == 0) {
@@ -383,7 +393,7 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
   TileCursor<SYM, BN> cursor;
   cursor.init(tiles_m, tiles_n);
   for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    const TileCoord tc = cursor.at(tile, tab);
+    const TileCoord tc = LIST ? listed_tile(tile_list, tile) : cursor.at(tile, tab);
 #pragma unroll
     for (int i = 0; i < NACC; ++i) sum[i] = 0.0f;
     // One chain per pass of the outer loop.  Its end is a structural wait<0>, so the compiler sees
@@ -479,19 +489,21 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
               if (col != dcol && (full || col < N)) mx = fmaxf(mx, v);
             } else if (!straddle || 8 * j + e >= diag + 8 * h) {
               mx = fmaxf(mx, v);
-              sm += v;
+              if (!LIST) sm += v;
             }
           }
         }
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
         mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-        if (EPI == TC_EPI_PLAIN) {
+        if (EPI == TC_EPI_PLAIN && !LIST) {
           sm += __shfl_xor_sync(0xffffffffu, sm, 1);
           sm += __shfl_xor_sync(0xffffffffu, sm, 2);
         }
         if ((lane & 3) == 0 && row < M) {
           if (EPI == TC_EPI_AFFINITY) {
             atomic_max_nonneg(rowmax_offdiag + row, mx);
+          } else if (LIST) {
+            atomic_max_nonneg(stat_rowmax + row_map[row], mx);
           } else {
             atomic_max_nonneg(stat_rowmax + row, mx);
             atomicAdd(stat_rowsum + row, (double)sm);
@@ -513,17 +525,19 @@ k_gemm_wgmma(const __grid_constant__ CUtensorMap map_a_hi,
             if ((full || r0 + 8 * h < M) && (!straddle || 8 * j + e > diag + 8 * h)) {
               const float v = sum[4 * j + 2 * h + e];
               mx = fmaxf(mx, v);
-              sm += v;
+              if (!LIST) sm += v;
             }
           }
 #pragma unroll
           for (int o = 4; o < 32; o <<= 1) {
             mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-            if (EPI == TC_EPI_PLAIN) sm += __shfl_xor_sync(0xffffffffu, sm, o);
+            if (EPI == TC_EPI_PLAIN && !LIST) sm += __shfl_xor_sync(0xffffffffu, sm, o);
           }
           if (lane < 4 && tr < N) {
             if (EPI == TC_EPI_AFFINITY) {
               atomic_max_nonneg(rowmax_offdiag + tr, mx);
+            } else if (LIST) {
+              atomic_max_nonneg(stat_rowmax + row_map[tr], mx);
             } else {
               atomic_max_nonneg(stat_rowmax + tr, mx);
               atomicAdd(stat_rowsum + tr, (double)sm);
@@ -682,7 +696,7 @@ static int launch(const sc_context* ctx, const __half* a_hi, const __half* a_lo,
   }
   kern<<<grid, NUM_THREADS, smem, st>>>(ah, al, bh, bl, tab, M, N, K, C, ldc, rowmax, diag_shift,
                                         pace, pace_kb, stat_rowmax, stat_rowsum, mirror, ldm,
-                                        aff_chunk_kb);
+                                        aff_chunk_kb, nullptr, nullptr, nullptr);
   sc::launched();
   SC_LAUNCH_CHECK();
   return 0;
@@ -726,6 +740,169 @@ int gemm_nt_wgmma(const sc_context* ctx, int epi, int precision, const __half* a
   if (precision == SC_GEMM_SPLIT2) SC_TC_LAUNCH(2, TC_EPI_PLAIN, 192);
   SC_TC_LAUNCH(1, TC_EPI_PLAIN, 192);
 #undef SC_TC_LAUNCH
+}
+
+// ---------------------------------------------------------------- bounded Diffuse (row maxima)
+// RowWiseNormalize after Diffuse needs max_j S_ij of S = Y Y^T, and Y >= 0.  For 256-column groups
+// g, S_ij = sum_g <y_i^g, y_j^g> <= sum_g |y_i^g| |y_j^g|, and every row's maximum is at least its
+// diagonal S_ii = |y_i|^2.  A tile of the (row-permuted) product whose bound
+//   u = sum_g max_{rows of the tile} |y^g| x max_{columns of the tile} |y^g|
+// lies below the smallest diagonal of its rows and columns, l, holds no row maximum of either.  With
+// the computed product within a factor (1 +- BOUND_EPS) of the exact one (DESIGN.md section 3), a
+// tile is skipped iff u (1 + eps) < l (1 - eps); tiles that straddle the diagonal are always
+// computed, so every S~_ii is.  u is accumulated in fp64 rounded up and l from diagonals rounded
+// down, so the rule holds in floating point as it does in exact arithmetic.
+constexpr int LIST_BN = 192;                       // the single-MMA Diffuse tile width
+constexpr double BOUND_EPS = 1.0 / 1024;           // valid for K <= 2^20
+constexpr int BOUND_MAX_K = 1 << 20;
+
+// Maxima of the group norms and minimum of the diagonal lower bounds over each block of R rows of
+// the permuted order (permuted row r is row perm[r]).
+__global__ void k_block_bounds(const float* __restrict__ norms, int G,
+                               const double* __restrict__ diag_lb, const int* __restrict__ perm,
+                               int n, int R, float* __restrict__ bmax, double* __restrict__ bmin) {
+  const int b = blockIdx.x;
+  const int r0 = b * R, r1 = min(n, r0 + R);
+  for (int g = threadIdx.x; g < G; g += blockDim.x) {
+    float m = 0.0f;
+    for (int r = r0; r < r1; ++r) m = fmaxf(m, norms[(int64_t)perm[r] * G + g]);
+    bmax[(int64_t)b * G + g] = m;
+  }
+  if (threadIdx.x < 32) {
+    double l = INFINITY;
+    for (int r = r0 + (int)threadIdx.x; r < r1; r += 32) l = fmin(l, diag_lb[perm[r]]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) l = fmin(l, __shfl_xor_sync(0xffffffffu, l, o));
+    if (threadIdx.x == 0) bmin[b] = l;
+  }
+}
+
+// One warp per (m, n) tile: flags[m tiles_n + n] = 1 iff the tile is computed.
+__global__ void k_tile_flags(const float* __restrict__ amax, const double* __restrict__ amin,
+                             const float* __restrict__ bmax, const double* __restrict__ bmin, int G,
+                             int tiles_m, int tiles_n, uint8_t* __restrict__ flags) {
+  const int64_t id = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (id >= (int64_t)tiles_m * tiles_n) return;
+  const int m = (int)(id / tiles_n), nb = (int)(id - (int64_t)m * tiles_n);
+  const int64_t row0 = (int64_t)m * BM, col0 = (int64_t)nb * LIST_BN;
+  bool keep;
+  if (col0 + LIST_BN - 1 < row0) {
+    keep = false;                                   // below the diagonal: never enumerated
+  } else if (col0 < row0 + BM) {
+    keep = true;                                    // straddles the diagonal
+  } else {
+    double u = 0.0;                                 // fp32 x fp32 is exact in fp64
+    for (int g = lane; g < G; g += 32)
+      u = __fma_ru((double)amax[(int64_t)m * G + g], (double)bmax[(int64_t)nb * G + g], u);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) u = __dadd_ru(u, __shfl_xor_sync(0xffffffffu, u, o));
+    const double l = fmin(amin[m], bmin[nb]);
+    keep = !(__dmul_ru(u, 1.0 + BOUND_EPS) < __dmul_rd(l, 1.0 - BOUND_EPS));
+  }
+  if (lane == 0) flags[id] = keep ? 1 : 0;
+}
+
+// One block: the flagged tiles in the rasterised order of the symmetric launch (TileCursor), packed
+// m << 16 | n, their number in *count and the number of upper tiles in *total.
+__global__ void k_tile_compact(const uint8_t* __restrict__ flags, int tiles_m, int tiles_n,
+                               uint32_t* __restrict__ list, int* __restrict__ count,
+                               int* __restrict__ total) {
+  __shared__ int warp_tot[32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  int base = 0, all = 0;
+  const int groups = (tiles_m + GROUP_M - 1) / GROUP_M;
+  for (int g = 0; g < groups; ++g) {
+    const int nb0 = sym_first_nblk<LIST_BN>(g);
+    const int span = (tiles_n - nb0) * GROUP_M;
+    for (int c0 = 0; c0 < span; c0 += blockDim.x) {
+      const int idx = c0 + (int)threadIdx.x;
+      bool valid = false, keep = false;
+      int m = 0, nb = 0;
+      if (idx < span) {
+        nb = nb0 + idx / GROUP_M;
+        const int mi = idx % GROUP_M;
+        valid = mi < sym_valid_mblocks<LIST_BN>(g, nb, tiles_m);
+        m = g * GROUP_M + mi;
+        keep = valid && flags[(int64_t)m * tiles_n + nb];
+      }
+      const unsigned bal = __ballot_sync(0xffffffffu, keep);
+      if (lane == 0) warp_tot[w] = __popc(bal);
+      __syncthreads();
+      int off = 0, tot = 0;
+      for (int i = 0; i < nw; ++i) {
+        const int v = warp_tot[i];
+        off += i < w ? v : 0;
+        tot += v;
+      }
+      if (keep) list[base + off + __popc(bal & ((1u << lane) - 1u))] = ((uint32_t)m << 16) | nb;
+      base += tot;
+      all += __syncthreads_count(valid);            // also the barrier before warp_tot is reused
+    }
+  }
+  if (threadIdx.x == 0) {
+    *count = base;
+    *total = all;
+  }
+}
+
+int diffuse_tile_list(const float* norms, int G, const double* diag_lb, const int* perm,
+                      int64_t n, uint32_t* list, int* count, int* total, cudaStream_t st) {
+  SC_REQUIRE(n > 0 && n <= BOUND_MAX_K && G == (n + 255) / 256,
+             "sc_diffuse_tile_list: n must lie in [1, 2^20] and G = ceil(n / 256)");
+  const int tiles_m = (int)((n + BM - 1) / BM), tiles_n = (int)((n + LIST_BN - 1) / LIST_BN);
+  Scratch amax, bmax, amin, bmin, flags;
+  SC_CUDA(amax.alloc(sizeof(float) * tiles_m * G, st));
+  SC_CUDA(bmax.alloc(sizeof(float) * tiles_n * G, st));
+  SC_CUDA(amin.alloc(sizeof(double) * tiles_m, st));
+  SC_CUDA(bmin.alloc(sizeof(double) * tiles_n, st));
+  SC_CUDA(flags.alloc((size_t)tiles_m * tiles_n, st));
+  k_block_bounds<<<tiles_m, 256, 0, st>>>(norms, G, diag_lb, perm, (int)n, BM, amax.as<float>(),
+                                          amin.as<double>());
+  k_block_bounds<<<tiles_n, 256, 0, st>>>(norms, G, diag_lb, perm, (int)n, LIST_BN,
+                                          bmax.as<float>(), bmin.as<double>());
+  const int64_t tiles = (int64_t)tiles_m * tiles_n;
+  k_tile_flags<<<(unsigned)((tiles + 7) / 8), 256, 0, st>>>(
+      amax.as<float>(), amin.as<double>(), bmax.as<float>(), bmin.as<double>(), G, tiles_m, tiles_n,
+      flags.as<uint8_t>());
+  k_tile_compact<<<1, 1024, 0, st>>>(flags.as<uint8_t>(), tiles_m, tiles_n, list, count, total);
+  sc::launched(4);
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
+int diffuse_rowmax_tiles(const sc_context* ctx, const __half* y_hi, int64_t ldh, int64_t n,
+                         const uint32_t* list, const int* count, const int* row_map,
+                         float* rowmax, cudaStream_t st) {
+  SC_REQUIRE(n > 0 && n <= BOUND_MAX_K, "sc_diffuse_rowmax_tiles: n must lie in [1, 2^20]");
+  constexpr int PREC = 1, BN = LIST_BN;
+  constexpr int STAGES = StageGeom<PREC, BN>::STAGES;
+  constexpr int STAGE_BYTES = StageGeom<PREC, BN>::BYTES;
+  CUtensorMap ah, bh;
+  if (int r = make_plane_map(&ah, y_hi, n, n, ldh, BM)) return r;
+  if (int r = make_plane_map(&bh, y_hi, n, n, ldh, BN)) return r;
+  const size_t smem = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+  SC_REQUIRE(smem <= ctx->smem_optin, "wgmma GEMM needs %zu B of shared memory", smem);
+  auto kern = k_gemm_wgmma<PREC, TC_EPI_PLAIN, true, BN, true>;
+  SC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  SC_CUDA(cudaMemsetAsync(rowmax, 0, sizeof(float) * n, st));
+  int grid = ctx->sm_count;
+  if (ctx->gemm_sm_limit > 0 && ctx->gemm_sm_limit < grid) grid = ctx->gemm_sm_limit;
+  // the tile count is on the device: pace whenever K is long enough (CTAs without a tile sign off
+  // their checkpoints, as in the last round of the enumerated launch)
+  unsigned int* pace = nullptr;
+  if (ctx->gemm_pace && (n + BK - 1) / BK >= 2 * PACE_KB) {
+    static std::atomic<unsigned int> pace_turn{0};
+    pace = ctx->gemm_pace + (pace_turn.fetch_add(1) % SC_GEMM_PACE_SLOTS);
+    SC_CUDA(cudaMemsetAsync(pace, 0, sizeof(unsigned int), st));
+  }
+  TileTable tab = {};
+  kern<<<grid, NUM_THREADS, smem, st>>>(ah, ah, bh, bh, tab, (int)n, (int)n, (int)n, nullptr, 0,
+                                        nullptr, 0, pace, PACE_KB, rowmax, nullptr, nullptr, 0, 1,
+                                        list, count, row_map);
+  sc::launched();
+  SC_LAUNCH_CHECK();
+  return 0;
 }
 
 }  // namespace sc

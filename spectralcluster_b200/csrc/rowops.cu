@@ -271,6 +271,71 @@ __global__ void k_row_stats(const float* __restrict__ a, int64_t n /*columns*/, 
   }
 }
 
+// ------------------------------------------------------------------ bounds of the Diffuse rows
+// One read of the fp16 plane of Y (non-negative, 256 threads per row, 8 columns per thread, so one
+// warp covers one 256-column group per step): per row the group norms |y_i^g| (fp64 sum of squares
+// rounded up, stored as fp32 rounded up), a lower bound of the diagonal |y_i|^2 of S = Y Y^T (fp64,
+// every addition rounded down; fp16 squares are exact in fp64, so it is the exact diagonal unless
+// the row spans more than 2^53 in magnitude) and the row sums c_i (fp64).
+constexpr int BOUND_GROUP = 256;
+
+__device__ __forceinline__ double warp_sum_rd(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = __dadd_rd(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+__global__ void __launch_bounds__(256) k_row_group_bounds(const __half* __restrict__ y, int64_t n,
+                                                          int64_t ldy, float* __restrict__ norms,
+                                                          int G, double* __restrict__ diag_lb,
+                                                          double* __restrict__ rowsum) {
+  __shared__ double red[32];
+  const int64_t i = blockIdx.x;
+  const __half* r = y + i * ldy;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  double lo = 0.0, s = 0.0;
+  for (int64_t c0 = 0; c0 < n; c0 += 256 * 8) {
+    const int64_t j = c0 + (int64_t)threadIdx.x * 8;
+    double up = 0.0;
+    if (j < n) {
+      const uint4 q = __ldg(reinterpret_cast<const uint4*>(r + j));
+      const __half* h = reinterpret_cast<const __half*>(&q);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const double v = (j + e < n) ? (double)__half2float(h[e]) : 0.0;
+        up = __fma_ru(v, v, up);
+        lo = __fma_rd(v, v, lo);
+        s += v;
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) up = __dadd_ru(up, __shfl_xor_sync(0xffffffffu, up, o));
+    const int64_t g = c0 / BOUND_GROUP + w;
+    if (lane == 0 && g < G) norms[i * G + g] = __double2float_ru(__dsqrt_ru(up));
+  }
+  lo = warp_sum_rd(lo);
+  __syncthreads();
+  if (lane == 0) red[w] = lo;
+  __syncthreads();
+  lo = (lane < 8) ? red[lane] : 0.0;
+  lo = warp_sum_rd(lo);
+  s = block_sum(s, red);
+  if (threadIdx.x == 0) {
+    diag_lb[i] = lo;
+    rowsum[i] = s;
+  }
+}
+
+// dst row r = src row perm[r] (fp16, whole rows of `cols` elements, cols % 8 == 0)
+__global__ void k_gather_rows_f16(const __half* __restrict__ src, int64_t lds,
+                                  const int* __restrict__ perm, int64_t cols,
+                                  __half* __restrict__ dst, int64_t ldd) {
+  const int64_t r = blockIdx.x;
+  const uint4* in = reinterpret_cast<const uint4*>(src + (int64_t)perm[r] * lds);
+  uint4* out = reinterpret_cast<uint4*>(dst + r * ldd);
+  for (int64_t j = threadIdx.x; j < cols / 8; j += blockDim.x) out[j] = __ldg(in + j);
+}
+
 // ------------------------------------------------------------------ single-cluster statistics
 // fallback_clusterer.check_single_cluster (fallback_clusterer.py:127-187) needs three reductions
 // of the affinity: its minimum (AllAffinity, :143), the minimum of the first super-diagonal
@@ -574,6 +639,34 @@ extern "C" int sc_scale_shift(sc_context* ctx, const float* x, int64_t ldx, int6
   SC_REQUIRE(n <= 65535, "sc_scale_shift: n too large for the element-wise grid");
   k_scale_shift<<<dim3((unsigned)((n + 255) / 256), (unsigned)n), 256, 0, as_stream(stream)>>>(
       x, ldx, n, row_scale, col_scale, alpha, beta, out, ldo); sc::launched();
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int sc_row_group_bounds(sc_context* ctx, const void* y_hi, int64_t n, int64_t ldy,
+                                   float* norms, int64_t groups, double* diag_lb, double* rowsum,
+                                   void* stream) {
+  SC_REQUIRE(ctx && y_hi && norms && diag_lb && rowsum && n > 0 &&
+             groups == (n + BOUND_GROUP - 1) / BOUND_GROUP, "sc_row_group_bounds: bad arguments");
+  SC_REQUIRE(vec_ok_f16(y_hi, ldy) && ldy >= n, "sc_row_group_bounds: y_hi needs a 16-byte aligned "
+             "base and ldy %% 8 == 0");
+  k_row_group_bounds<<<(unsigned)n, 256, 0, as_stream(stream)>>>(
+      (const __half*)y_hi, n, ldy, norms, (int)groups, diag_lb, rowsum);
+  sc::launched();
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int sc_gather_rows_f16(sc_context* ctx, const void* src, int64_t lds, const int* perm,
+                                  int64_t rows, int64_t cols, void* dst, int64_t ldd,
+                                  void* stream) {
+  SC_REQUIRE(ctx && src && perm && dst && rows > 0 && cols > 0 && cols % 8 == 0 && cols <= lds &&
+             cols <= ldd, "sc_gather_rows_f16: bad arguments");
+  SC_REQUIRE(vec_ok_f16(src, lds) && vec_ok_f16(dst, ldd),
+             "sc_gather_rows_f16: 16-byte aligned bases and leading dimensions %% 8 == 0");
+  k_gather_rows_f16<<<(unsigned)rows, 256, 0, as_stream(stream)>>>(
+      (const __half*)src, lds, perm, cols, (__half*)dst, ldd);
+  sc::launched();
   SC_LAUNCH_CHECK();
   return 0;
 }

@@ -38,11 +38,27 @@ FACTORED_PANEL_BYTES = 1 << 30
 # Panel origins sit on the affinity's 128-row tiles (which also aligns them with the 64-row tiles
 # of the threshold pass and the 32-row bands of the blur); the blur reads 4 rows on either side.
 PANEL_ALIGN, BLUR_HALO = 128, 4
+# Bounded Diffuse (sc_diffuse_tile_list): the column groups of its row bounds, its output tile, and
+# the row order -- cosine k-means with this many clusters and passes on the rows' group-norm
+# profiles (the order only decides which tiles are skipped, never a value).
+BOUND_GROUP_COLS, LIST_BM, LIST_BN = 256, 128, 192
+BOUND_ORDER_CLUSTERS, BOUND_ORDER_ITERS = 16, 20
+# predict() takes the bounded Diffuse from this N (tools/time_bounded_diffuse.py, H100 80GB HBM3,
+# 700 W): at 16,384 its fixed costs (mostly the row order, 5.5 ms) leave it 25 % slower than the
+# storing Diffuse + stored solve (11.7 against 9.4 ms); at 32,768 it is 40 % faster (33 against 56).
+BOUNDED_FROM = 32768
 
 
 def stored_route_peak_bytes(n: int) -> int:
   """Peak device bytes of predict()'s stored route at n, computed from shapes."""
   return STORED_ROUTE_BYTES_PER_ELEMENT * n * round_up(n, 64)
+
+
+def bounded_tile_count(n: int) -> int:
+  """Tiles of the symmetric single-MMA Diffuse launch (those that reach the upper triangle)."""
+  tiles_n = -(-n // LIST_BN)
+  return sum(tiles_n - max(0, -(-(LIST_BM * m - LIST_BN + 1) // LIST_BN))
+             for m in range(-(-n // LIST_BM)))
 
 
 def panel_rows_for(n: int) -> int:
@@ -368,6 +384,61 @@ class Engine:
               hi.stride(0), n, None, 0, _ptr(mx), _ptr(sm), self.stream)
     return mx, sm
 
+  def row_group_bounds(self, hi, n):
+    """(norms fp32 [n, G], diagonal lower bounds fp64, row sums fp64) of the fp16 plane `hi`; the
+    row sums carry a zero pad to an even length, the block product's operand alignment."""
+    t = torch()
+    g = -(-n // BOUND_GROUP_COLS)
+    norms = t.empty((n, g), dtype=t.float32, device=self.device)
+    diag, c = self.vector(n), self.vector(round_up(n, 2), zero=True)
+    self.call("sc_row_group_bounds", _ptr(hi), n, hi.stride(0), _ptr(norms), g, _ptr(diag), _ptr(c),
+              self.stream)
+    return norms, diag, c
+
+  def bound_order(self, norms):
+    """Row order of the bounded Diffuse: stable sort of the cosine k-means labels of the profiles
+    (device int32).  Profiles k-means cannot seed (all rows alike) keep the natural order."""
+    t = torch()
+    n = int(norms.shape[0])
+    try:
+      labels, _ = self.kmeans(norms.double(), BOUND_ORDER_CLUSTERS, 0, BOUND_ORDER_ITERS)
+      perm = np.argsort(labels, kind="stable").astype(np.int32)
+    except ValueError:
+      perm = np.arange(n, dtype=np.int32)
+    return t.from_numpy(perm).to(self.device)
+
+  def rowmax_tiles(self, hi, n, norms, diag, perm):
+    """Row maxima (fp32) of S = hi hi^T from the tiles of the product of hi[perm] that can hold
+    one, and (computed, total) tile counts as a device int32 [2]."""
+    t = torch()
+    yp = t.empty_like(hi)
+    self.call("sc_gather_rows_f16", _ptr(hi), hi.stride(0), _ptr(perm), n, hi.shape[1], _ptr(yp),
+              yp.stride(0), self.stream)
+    tiles = t.empty(-(-n // LIST_BM) * -(-n // LIST_BN), dtype=t.int32, device=self.device)
+    counts = t.empty(2, dtype=t.int32, device=self.device)
+    self.call("sc_diffuse_tile_list", _ptr(norms), int(norms.shape[1]), _ptr(diag), _ptr(perm), n,
+              _ptr(tiles), _ptr(counts), _ptr(counts[1:]), self.stream)
+    mx = self.vector(n, t.float32)
+    self.call("sc_diffuse_rowmax_tiles", _ptr(yp), yp.stride(0), n, _ptr(tiles), _ptr(counts),
+              _ptr(perm), _ptr(mx), self.stream)
+    del yp
+    return mx, counts
+
+  def bounded_diffuse(self, n, hi, want_max=True):
+    """Statistics of S = Y Y^T (Y >= 0 and bitwise symmetric, `hi` its fp16 plane), S never formed:
+    (rowmax fp32 or None, rowsum fp64, tile counts).  rowsum = Y (Y 1) by two passes over Y; the
+    row maxima, when wanted, from the bounded tile list (bit for bit those of sc_diffuse).  The
+    counts are an int32 tensor [2] (computed, total): on the device, or on the host (0 computed)
+    when no GEMM runs."""
+    t = torch()
+    norms, diag, c = self.row_group_bounds(hi, n)
+    rowsum = t.empty((1, n), dtype=t.float64, device=self.device)
+    self.block_product_f16(hi, n, n, c.view(1, -1), 1, rowsum)
+    if not want_max:
+      return None, rowsum.view(n), t.tensor([0, bounded_tile_count(n)], dtype=t.int32)
+    mx, counts = self.rowmax_tiles(hi, n, norms, diag, self.bound_order(norms))
+    return mx, rowsum.view(n), counts
+
   # ---- row panels of the factored route
   def normalized_planes(self, x_dev):
     """Split fp16 planes of the row-normalised embeddings (the affinity GEMM's operands)."""
@@ -599,13 +670,15 @@ class Refined:
   `symmetric` tells whether S is symmetric (up to rounding).  On the factored route S is not
   stored: `s` is None and S = y_hi y_hi^T with y_hi the fp16 hi plane of Y."""
 
-  def __init__(self, s, n, symmetric, row_scale=None, rowsum=None, y_hi=None):
+  def __init__(self, s, n, symmetric, row_scale=None, rowsum=None, y_hi=None, tiles=None):
     self.s = s
     self.n = n
     self.symmetric = symmetric
     self.row_scale = row_scale
     self.rowsum = rowsum      # fp64 row sums of S when the Diffuse epilogue produced them
     self.y_hi = y_hi
+    # bounded Diffuse (stored front end): its (computed, total) tile counts, an int32 tensor [2]
+    self.tiles = tiles
 
 
 def factored_sequence_ok(eng: Engine, options) -> bool:
@@ -688,7 +761,7 @@ class FactoredAffinity:
 
 
 def run_refinement(eng: Engine, a, n: int, options, crop_vector=None, a_symmetric=True,
-                   diffuse_precision=None) -> Refined:
+                   diffuse_precision=None, bounded=False) -> Refined:
   """Apply options.refinement_sequence to the device affinity `a`.
 
   Fusions (all exact restatements, SURVEY.md A.3):
@@ -697,6 +770,8 @@ def run_refinement(eng: Engine, a, n: int, options, crop_vector=None, a_symmetri
            emitting fp16 planes directly when Diffuse follows;
     RowWiseNormalize as the last operator -> kept as a row scaling for the eigensolver.
   Anything else runs operator by operator.
+  `bounded` (the caller checked the scope: a single-MMA Diffuse closing the fused chain): S is not
+  stored; the result carries Y_hi, the row sums Y (Y 1) and the bounded Diffuse's row maxima.
   """
   from . import refinement as rf
   names = list(options.refinement_sequence or [])
@@ -707,6 +782,7 @@ def run_refinement(eng: Engine, a, n: int, options, crop_vector=None, a_symmetri
   cur_is_planes_only = False
   row_scale = None
   stats = None           # (rowmax fp32, rowsum fp64) of `cur` straight from the Diffuse epilogue
+  y_hi = tiles = None    # the bounded Diffuse's operand and tile counts
   i = 0
   while i < len(names):
     name = names[i]
@@ -770,12 +846,15 @@ def run_refinement(eng: Engine, a, n: int, options, crop_vector=None, a_symmetri
       tail = names[i + 1:]
       fuse_stats = (tail in ([], [RN.RowWiseNormalize]) and
                     eng.gemm_engine(n) == nat.GEMM_TCGEN05)
-      if planes is not None:
+      if bounded and fuse_stats and planes is not None and planes[1] is None:
+        mx, sm, tiles = eng.bounded_diffuse(n, planes[0], want_max=tail == [RN.RowWiseNormalize])
+        y_hi, cur = planes[0], None
+      elif planes is not None:
         cur, mx, sm = eng.diffuse(n, hi=planes[0], lo=planes[1], want_stats=fuse_stats,
                                   precision=diffuse_precision)
       else:
         cur, mx, sm = eng.diffuse(n, y=cur, want_stats=fuse_stats, precision=diffuse_precision)
-      stats = (mx, sm) if mx is not None else None
+      stats = (mx, sm) if sm is not None else None
       planes, cur_is_planes_only, sym = None, False, True
       i += 1
       continue
@@ -820,7 +899,8 @@ def run_refinement(eng: Engine, a, n: int, options, crop_vector=None, a_symmetri
     else:
       raise ValueError("Unknown refinement operation: {}".format(name))
     i += 1
-  return Refined(cur, n, sym, row_scale, stats[1] if stats is not None else None)
+  return Refined(cur, n, sym, row_scale, stats[1] if stats is not None else None, y_hi=y_hi,
+                 tiles=tiles)
 
 
 def _materialise_scale(eng: Engine, s, n: int, row_scale):

@@ -134,7 +134,9 @@ class SpectralClusterer:
       refined = dev.run_refinement(eng, affinity.matrix, n, self.refinement_options,
                                    crop_vector=affinity.crop_vector,
                                    a_symmetric=affinity.symmetric,
-                                   diffuse_precision=eng.diffuse_precision_for(n))
+                                   diffuse_precision=eng.diffuse_precision_for(n),
+                                   bounded=affinity.symmetric and
+                                   self._bounded_route(eng, n, constraint_matrix))
     if (self.constraint_options and not self.constraint_options.apply_before_refinement and
         constraint_matrix is not None):
       # constraint on the refined affinity (spectral_clusterer.py:137-142)
@@ -168,8 +170,10 @@ class SpectralClusterer:
         w, v, stats = arnoldi.eig_extremal_device(eng, *op, not descend, limit, n_vectors)
         top_solve = lambda: arnoldi.eig_extremal_device(eng, *op, False, 1, 0)[0]
     elif refined.y_hi is not None:
-      # factored route (its scope guarantees lanczos_fits): S = Y_hi Y_hi^T is never stored
-      solver = "lanczos-factored"
+      # factored operator (the scope of both routes guarantees lanczos_fits): S = Y_hi Y_hi^T is
+      # never stored.  `solver` names the route's choice: one Lanczos solve after the bounded
+      # Diffuse of the stored front end, "lanczos-factored" on the panel route.
+      solver = "lanczos" if refined.tiles is not None else "lanczos-factored"
       fop = (refined.y_hi,) + op[1:]
       w, v, stats = eng.eigh_factored(*fop, which, limit, n_vectors)
       stats = stats.tolist()
@@ -214,24 +218,39 @@ class SpectralClusterer:
     k, gap = counted or self._count_clusters(w, descend, top)
     self.last_details = dict(eigenvalues=np.array(w[:limit]), n_clusters_raw=k, max_gap=gap,
                              solver=solver, lanczos_stats=stats)
+    if refined.tiles is not None:
+      computed, total = refined.tiles.tolist()
+      self.last_details["diffuse"] = dict(tiles=computed, of=total, operator="factored")
     return w, v, k, gap
 
-  def _factored_route(self, eng, n: int, constraint_matrix=None) -> bool:
-    """Whether predict() on n embeddings takes the factored route: the stored route's peak
-    (computed from shapes) exceeds eng.factored_above_bytes and every option is one the factored
-    route serves; any other call keeps the stored route."""
-    if dev.stored_route_peak_bytes(n) <= eng.factored_above_bytes:
-      return False
+  def _lanczos_scope(self, eng, n: int, constraint_matrix=None) -> bool:
+    """The options both routes that never store S serve: the default affinity, the fused chain
+    closed by a single-MMA Diffuse (dev.factored_sequence_ok), no constraint, and one Lanczos solve
+    (bounded max_clusters < LANCZOS_MAX_PAIRS that lanczos_fits)."""
     limit = (self.max_clusters or 0) + 1
     return (self.affinity_function is utils.compute_affinity_matrix and
             self.min_clusters != 1 and (self.min_clusters or 0) <= limit and
             not (self.constraint_options and constraint_matrix is not None) and
             self.max_clusters is not None and self.max_clusters < LANCZOS_MAX_PAIRS and
-            n > limit and n > eng.dense_eig_max and lanczos_fits(n, limit) and
             self.autotune_group is None and
+            dev.factored_sequence_ok(eng, self.refinement_options) and
+            n > limit and n > eng.dense_eig_max and lanczos_fits(n, limit) and
             eng.gemm_engine(n) == nat.GEMM_TCGEN05 and
-            eng.diffuse_precision_for(n) == nat.GEMM_SINGLE and
-            dev.factored_sequence_ok(eng, self.refinement_options))
+            eng.diffuse_precision_for(n) == nat.GEMM_SINGLE)
+
+  def _factored_route(self, eng, n: int, constraint_matrix=None) -> bool:
+    """Whether predict() on n embeddings takes the factored route: the stored route's peak
+    (computed from shapes) exceeds eng.factored_above_bytes and every option is one the factored
+    route serves; any other call keeps the stored route."""
+    return (self._lanczos_scope(eng, n, constraint_matrix) and
+            dev.stored_route_peak_bytes(n) > eng.factored_above_bytes)
+
+  def _bounded_route(self, eng, n: int, constraint_matrix=None) -> bool:
+    """Whether the stored front end (a resident affinity) replaces the storing Diffuse and the
+    stored Lanczos solve by the bounded Diffuse and a Lanczos solve on the factored operator: the
+    calls of _lanczos_scope from N = dev.BOUNDED_FROM that do not take the factored route."""
+    return (n >= dev.BOUNDED_FROM and self._lanczos_scope(eng, n, constraint_matrix) and
+            dev.stored_route_peak_bytes(n) <= eng.factored_above_bytes)
 
   def _count_clusters(self, eigenvalues, descend: bool, max_eigenvalue=None):
     """utils.compute_number_of_clusters with this clusterer's options -> (k, max gap); only a
