@@ -49,6 +49,8 @@ enum sc_gemm_precision {
   SC_GEMM_SPLIT2 = 2     /* (hi+lo)*hi : B rounded to fp16, zero-mean 2^-12 per product */
 };
 enum sc_which_end { SC_EIG_LARGEST = 0, SC_EIG_SMALLEST = 1 };
+/* element type of an input matrix (F32 / F64 agree with the x_is_f64 flags of older entries) */
+enum sc_dtype { SC_DTYPE_F32 = 0, SC_DTYPE_F64 = 1, SC_DTYPE_F16 = 2, SC_DTYPE_BF16 = 3 };
 
 typedef struct sc_context sc_context;
 
@@ -73,6 +75,14 @@ int sc_context_set_gemm_sm_limit(sc_context* ctx, int sms);
 int sc_normalize_rows(sc_context* ctx, const void* x, int x_is_f64, int64_t n, int64_t d,
                       int64_t ldx, float* xn, int64_t ldxn, void* hi, void* lo, int64_t ldh,
                       void* stream);
+
+/* sc_normalize_rows on rows of any sc_dtype (x_dtype), read in place with row stride ldx and unit
+ * column stride.  Each element widens exactly to fp64, so fp16 rows give bit for bit the outputs
+ * of sc_normalize_rows on their fp64 upcast, and bf16 rows those of their fp32 upcast
+ * (SpectralClusterer.predict on a CUDA tensor: no widened N x d staging copy). */
+int sc_normalize_rows_typed(sc_context* ctx, const void* x, int x_dtype, int64_t n, int64_t d,
+                            int64_t ldx, float* xn, int64_t ldxn, void* hi, void* lo,
+                            int64_t ldh, void* stream);
 
 /* A = (Xn Xn^T + 1) / 2 (utils.py:35-39).  engine TCGEN05 reads the split planes,
  * engine SIMT reads xn.  If rowmax_offdiag != NULL it receives max_j!=i A[i,j] clamped at 0
@@ -516,6 +526,18 @@ int sc_cosine_distances_f64(sc_context* ctx, const void* x, int x_is_f64, int64_
  * in the merged cluster).  dist is overwritten.  SYNCHRONOUS. */
 int sc_complete_linkage(sc_context* ctx, double* dist, int64_t n, int64_t ldd, int64_t* merge_xy,
                         double* merge_dist, int64_t* merge_size, void* stream);
+
+/* ---- utils.get_cluster_centroids (reference utils.py:159-177) ---------------------------------
+ * The cluster centroids of the max_spectral_size pre-clustering on the device.  x is [n,d] fp32
+ * (x_is_f64=0) or fp64 (=1) with row stride ldx and unit column stride; labels are n int64 ids
+ * (device).  out [k, ldo] fp64 receives, per id c in [0, k), the sum of the rows labelled c
+ * divided by their count: np.add.at into np.zeros fp64 sums, divided by np.bincount, bit for bit
+ * (each (cluster, column) is a sequential fp64 sum in increasing row index, after a stable
+ * counting sort of the rows by id).  An id with no row gives a NaN row; ids outside [0, k) are
+ * skipped.  n < 2^31. */
+int sc_cluster_centroids(sc_context* ctx, const void* x, int x_is_f64, int64_t n, int64_t d,
+                         int64_t ldx, const int64_t* labels, int64_t k, double* out, int64_t ldo,
+                         void* stream);
 
 /* ---- AgglomerativeClustering(metric="cosine", linkage="average", distance_threshold=t) -------
  * The single-cluster check of SingleClusterCondition.FallbackClusterer with

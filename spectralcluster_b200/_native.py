@@ -33,6 +33,8 @@ PROTOTYPES = {
     "sc_context_set_gemm_sm_limit": [c_ptr, c_int],
     "sc_normalize_rows": [c_ptr, c_ptr, c_int, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr, c_ptr,
                           c_i64, c_ptr],
+    "sc_normalize_rows_typed": [c_ptr, c_ptr, c_int, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr,
+                                c_ptr, c_i64, c_ptr],
     "sc_affinity_cosine": [c_ptr, c_int, c_int, c_ptr, c_i64, c_ptr, c_ptr, c_i64, c_i64, c_i64,
                            c_ptr, c_i64, c_ptr, c_ptr],
     "sc_crop_diagonal": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr],
@@ -126,6 +128,8 @@ PROTOTYPES = {
                   c_ptr, c_ptr, c_ptr],
     "sc_cosine_distances_f64": [c_ptr, c_ptr, c_int, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr,
                                 c_ptr],
+    "sc_cluster_centroids": [c_ptr, c_ptr, c_int, c_i64, c_i64, c_i64, c_ptr, c_i64, c_ptr, c_i64,
+                             c_ptr],
     "sc_complete_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_average_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_gmm_band_pass": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_int, c_ptr, c_ptr, c_ptr, c_ptr],
@@ -141,6 +145,7 @@ GEMM_TCGEN05, GEMM_SIMT = 0, 1
 GEMM_SPLIT3, GEMM_SINGLE, GEMM_SPLIT2 = 0, 1, 2
 ABI_VERSION = 2
 EIG_LARGEST, EIG_SMALLEST = 0, 1
+DTYPE_F32, DTYPE_F64, DTYPE_F16, DTYPE_BF16 = 0, 1, 2, 3
 
 _lib = None
 _lock = threading.Lock()

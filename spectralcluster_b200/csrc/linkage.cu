@@ -8,6 +8,9 @@
 //                      a row scan split across the grid (one CTA per SM), a grid barrier, and a
 //                      redundant reduction of the per-CTA minima in every CTA; a merge adds a
 //                      row + column update (the linkage's Lance-Williams rule) and one more barrier.
+// and the centroids of the clusters found (utils.get_cluster_centroids, max_spectral_size):
+//   k_centroid_order   stable counting sort of the row indices by cluster id, one warp
+//   k_centroid_sums    per (cluster, column): fp64 sum of the members in row order, over the count
 #include "common.cuh"
 
 #include <climits>
@@ -343,4 +346,101 @@ extern "C" int sc_average_linkage(sc_context* ctx, double* dist, int64_t n, int6
                                   void* stream) {
   return nn_chain_linkage<Linkage::Average>("sc_average_linkage", ctx, dist, n, ldd, merge_xy,
                                             merge_dist, merge_size, stream);
+}
+
+// ---- utils.get_cluster_centroids: np.add.at into fp64 sums, then division by np.bincount ----------
+namespace {
+
+// One warp walks the labels 32 at a time.  Lanes that hold the same id find each other with
+// __match_any_sync; the lowest of them moves the id's cursor past all of them, and each lane's
+// rank among them is the count of lower lanes, so every cluster lists its rows in increasing order.
+// Pass 1 counts, a warp scan turns counts into offsets, pass 2 scatters.  Ids outside [0, k) are
+// skipped.  off has k + 1 entries, cur k.
+__global__ void __launch_bounds__(32)
+k_centroid_order(const int64_t* __restrict__ labels, int64_t n, int64_t k, int64_t* off,
+                 int64_t* cur, int* perm) {
+  const int lane = threadIdx.x;
+  const unsigned lower = (1u << lane) - 1u;
+  for (int64_t c = lane; c < k; c += 32) cur[c] = 0;
+  __syncwarp();
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int64_t base = 0; base < n; base += 32) {
+      const int64_t i = base + lane;
+      const int64_t c = i < n ? labels[i] : -1;
+      const bool valid = c >= 0 && c < k;
+      const unsigned same = __match_any_sync(0xffffffffu, valid ? c : (int64_t)-1);
+      if (valid) {
+        const int64_t at = cur[c];
+        if (pass == 1) perm[at + __popc(same & lower)] = (int)i;
+        __syncwarp(same);
+        if ((same & lower) == 0) cur[c] = at + __popc(same);
+      }
+      __syncwarp();
+    }
+    if (pass == 0) {
+      // off = exclusive prefix sum of the counts; the cursors restart at the offsets
+      int64_t carry = 0;
+      for (int64_t c0 = 0; c0 < k; c0 += 32) {
+        const int64_t c = c0 + lane;
+        const int64_t v = c < k ? cur[c] : 0;
+        int64_t incl = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const int64_t u = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += u;
+        }
+        if (c < k) off[c] = cur[c] = carry + incl - v;
+        carry += __shfl_sync(0xffffffffu, incl, 31);
+      }
+      if (lane == 0) off[k] = carry;
+      __syncwarp();
+    }
+  }
+}
+
+// Block (cluster c, 128 columns): sequential fp64 adds of the members in increasing row index,
+// starting from 0.0 as np.add.at does into np.zeros, then one division by the member count (0 / 0
+// = NaN for an id with no member, as numpy gives).
+template <typename T>
+__global__ void __launch_bounds__(128)
+k_centroid_sums(const T* __restrict__ x, int64_t d, int64_t ldx, const int64_t* __restrict__ off,
+                const int* __restrict__ perm, double* __restrict__ out, int64_t ldo) {
+  const int64_t c = blockIdx.x;
+  const int64_t j = (int64_t)blockIdx.y * blockDim.x + threadIdx.x;
+  if (j >= d) return;
+  const int64_t b = off[c], e = off[c + 1];
+  double s = 0.0;
+#pragma unroll 8
+  for (int64_t r = b; r < e; ++r) s += (double)x[(int64_t)perm[r] * ldx + j];
+  out[c * ldo + j] = s / (double)(e - b);
+}
+
+}  // namespace
+
+extern "C" int sc_cluster_centroids(sc_context* ctx, const void* x, int x_is_f64, int64_t n,
+                                    int64_t d, int64_t ldx, const int64_t* labels, int64_t k,
+                                    double* out, int64_t ldo, void* stream) {
+  SC_REQUIRE(ctx && x && labels && out && n > 0 && d > 0 && k > 0 && ldo >= d &&
+             (n == 1 || ldx >= d), "sc_cluster_centroids: bad arguments");
+  SC_REQUIRE(n <= INT_MAX && k <= INT_MAX && (d + 127) / 128 <= 65535,
+             "sc_cluster_centroids: n = %lld, d = %lld or k = %lld is too large", (long long)n,
+             (long long)d, (long long)k);
+  cudaStream_t st = as_stream(stream);
+  Scratch off, cur, perm;
+  SC_CUDA(off.alloc(sizeof(int64_t) * (k + 1), st));
+  SC_CUDA(cur.alloc(sizeof(int64_t) * k, st));
+  SC_CUDA(perm.alloc(sizeof(int) * n, st));
+  k_centroid_order<<<1, 32, 0, st>>>(labels, n, k, off.as<int64_t>(), cur.as<int64_t>(),
+                                     perm.as<int>());
+  SC_LAUNCH_CHECK();
+  const dim3 grid((unsigned)k, (unsigned)((d + 127) / 128));
+  if (x_is_f64)
+    k_centroid_sums<double><<<grid, 128, 0, st>>>((const double*)x, d, ldx, off.as<int64_t>(),
+                                                  perm.as<int>(), out, ldo);
+  else
+    k_centroid_sums<float><<<grid, 128, 0, st>>>((const float*)x, d, ldx, off.as<int64_t>(),
+                                                 perm.as<int>(), out, ldo);
+  SC_LAUNCH_CHECK();
+  launched(2);
+  return 0;
 }

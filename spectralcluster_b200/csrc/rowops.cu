@@ -3,7 +3,7 @@
 // warp-shuffle reductions, second touch of a row served from L2.
 //
 // Reference operators replaced (file:line under /root/reference/spectralcluster):
-//   utils.py:32-33        row L2 normalisation          -> k_normalize_rows
+//   utils.py:32-33        row L2 normalisation          -> k_normalize_rows (fp16/bf16/fp32/fp64 rows)
 //   refinement.py:145-151 CropDiagonal                  -> k_crop_diagonal
 //   refinement.py:182-210 RowWiseThreshold              -> k_row_threshold (+ radix select)
 //   refinement.py:219-226 Symmetrize                    -> k_symmetrize
@@ -11,9 +11,18 @@
 //   laplacian.py:24-60    compute_laplacian             -> k_laplacian
 #include "common.cuh"
 
+#include <cuda_bf16.h>
+
 namespace sc {
 
 // ------------------------------------------------------------------ normalise rows
+// Every input dtype widens exactly to fp64, so an fp16 row gives what its fp64 upcast gives and a
+// bf16 row what its fp32 upcast gives.
+__device__ __forceinline__ double to_f64(float v) { return (double)v; }
+__device__ __forceinline__ double to_f64(double v) { return v; }
+__device__ __forceinline__ double to_f64(__half v) { return (double)__half2float(v); }
+__device__ __forceinline__ double to_f64(__nv_bfloat16 v) { return (double)__bfloat162float(v); }
+
 template <typename T>
 __global__ void k_normalize_rows(const T* __restrict__ x, int64_t n, int64_t d, int64_t ldx,
                                  float* __restrict__ xn, int64_t ldxn, __half* __restrict__ hi,
@@ -24,13 +33,13 @@ __global__ void k_normalize_rows(const T* __restrict__ x, int64_t n, int64_t d, 
   const T* r = x + row * ldx;
   double ss = 0.0;
   for (int64_t j = lane; j < d; j += 32) {
-    const double v = (double)r[j];
+    const double v = to_f64(r[j]);
     ss += v * v;
   }
   ss = warp_sum(ss);
   const double nrm = sqrt(ss);
   for (int64_t j = lane; j < d; j += 32) {
-    const float f = (float)((double)r[j] / nrm);
+    const float f = (float)(to_f64(r[j]) / nrm);
     if (xn) xn[row * ldxn + j] = f;
     if (hi) {
       __half h, l;
@@ -480,22 +489,46 @@ int crop_diagonal_rows(const float* a, int64_t n, int64_t lda, int64_t row_begin
 // ====================================================================== C ABI
 using namespace sc;
 
-extern "C" int sc_normalize_rows(sc_context* ctx, const void* x, int x_is_f64, int64_t n,
-                                 int64_t d, int64_t ldx, float* xn, int64_t ldxn, void* hi,
-                                 void* lo, int64_t ldh, void* stream) {
+extern "C" int sc_normalize_rows_typed(sc_context* ctx, const void* x, int x_dtype, int64_t n,
+                                       int64_t d, int64_t ldx, float* xn, int64_t ldxn, void* hi,
+                                       void* lo, int64_t ldh, void* stream) {
   SC_REQUIRE(ctx && x && n > 0 && d > 0, "sc_normalize_rows: bad arguments");
   SC_REQUIRE((hi == nullptr) == (lo == nullptr), "sc_normalize_rows: hi/lo must come together");
   const int warps = 8;
   const unsigned grid = (unsigned)((n + warps - 1) / warps);
-  if (x_is_f64)
-    k_normalize_rows<double><<<grid, warps * 32, 0, as_stream(stream)>>>(
-        (const double*)x, n, d, ldx, xn, ldxn, (__half*)hi, (__half*)lo, ldh);
-  else
-    k_normalize_rows<float><<<grid, warps * 32, 0, as_stream(stream)>>>(
-        (const float*)x, n, d, ldx, xn, ldxn, (__half*)hi, (__half*)lo, ldh);
+  cudaStream_t st = as_stream(stream);
+  __half* h = (__half*)hi;
+  __half* l = (__half*)lo;
+  switch (x_dtype) {
+    case SC_DTYPE_F32:
+      k_normalize_rows<float><<<grid, warps * 32, 0, st>>>((const float*)x, n, d, ldx, xn, ldxn,
+                                                            h, l, ldh);
+      break;
+    case SC_DTYPE_F64:
+      k_normalize_rows<double><<<grid, warps * 32, 0, st>>>((const double*)x, n, d, ldx, xn, ldxn,
+                                                             h, l, ldh);
+      break;
+    case SC_DTYPE_F16:
+      k_normalize_rows<__half><<<grid, warps * 32, 0, st>>>((const __half*)x, n, d, ldx, xn, ldxn,
+                                                             h, l, ldh);
+      break;
+    case SC_DTYPE_BF16:
+      k_normalize_rows<__nv_bfloat16><<<grid, warps * 32, 0, st>>>(
+          (const __nv_bfloat16*)x, n, d, ldx, xn, ldxn, h, l, ldh);
+      break;
+    default:
+      SC_REQUIRE(false, "sc_normalize_rows_typed: unknown dtype %d", x_dtype);
+  }
   sc::launched();
   SC_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int sc_normalize_rows(sc_context* ctx, const void* x, int x_is_f64, int64_t n,
+                                 int64_t d, int64_t ldx, float* xn, int64_t ldxn, void* hi,
+                                 void* lo, int64_t ldh, void* stream) {
+  return sc_normalize_rows_typed(ctx, x, x_is_f64 ? SC_DTYPE_F64 : SC_DTYPE_F32, n, d, ldx, xn,
+                                 ldxn, hi, lo, ldh, stream);
 }
 
 extern "C" int sc_crop_diagonal(sc_context* ctx, const float* a, int64_t n, int64_t lda,

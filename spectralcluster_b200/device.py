@@ -97,6 +97,46 @@ def round_up(x: int, m: int) -> int:
   return (x + m - 1) // m * m
 
 
+def dtype_code(x) -> int:
+  """The sc_dtype of a device tensor that sc_normalize_rows_typed reads."""
+  t = torch()
+  return {t.float32: nat.DTYPE_F32, t.float64: nat.DTYPE_F64, t.float16: nat.DTYPE_F16,
+          t.bfloat16: nat.DTYPE_BF16}[x.dtype]
+
+
+def device_embeddings(x):
+  """A CUDA tensor handed to predict() as embeddings -> the tensor predict() reads: detached,
+  float16 / bfloat16 / float32 / float64 (anything else widened to float64, as host arrays are),
+  with unit column stride and rows that do not overlap (anything else made contiguous once)."""
+  t = torch()
+  x = x.detach()
+  if x.dtype not in (t.float16, t.bfloat16, t.float32, t.float64):
+    x = x.to(t.float64)
+  n, d = int(x.shape[0]), int(x.shape[1])
+  if (d > 1 and x.stride(1) != 1) or (n > 1 and x.stride(0) < d):
+    x = x.contiguous()
+  return x
+
+
+def host_twin(x) -> np.ndarray:
+  """The ndarray a CUDA tensor stands for: x.cpu().numpy(), through float32 for bfloat16 (exact),
+  which numpy lacks.  Only where the reference hands the embeddings to user code."""
+  t = torch()
+  return (x.float() if x.dtype == t.bfloat16 else x).detach().cpu().numpy()
+
+
+def twin(x):
+  """A device tensor as fp32 / fp64 in the dtype its host twin reaches predict()'s arithmetic in:
+  float16 rows widen to float64 (predict() widens an fp16 ndarray so), bfloat16 rows to float32 (the
+  twin of a bf16 tensor is its exact fp32 upcast); fp32 / fp64 tensors are returned as they are."""
+  t = torch()
+  if x.dtype == t.float16:
+    return x.to(t.float64)
+  if x.dtype == t.bfloat16:
+    return x.to(t.float32)
+  return x
+
+
 def blur_radius(sigma: float) -> int:
   """scipy.ndimage.gaussian_filter's radius int(truncate * sigma + 0.5), truncate = 4; sigma <=
   1e-15 copies the input (radius 0).  The blur kernels apply the same rule."""
@@ -206,6 +246,8 @@ class Engine:
       "sc_affinity_stats": "fallback_clusterer.check_single_cluster",
       "sc_gmm_band_pass": "fallback_clusterer.check_single_cluster",
       "sc_constraint_combine": "constraint.adjust_affinity", "sc_scale_shift": "constraint.adjust_affinity",
+      "sc_normalize_rows_typed": "utils.compute_affinity_matrix",
+      "sc_cluster_centroids": "utils.get_cluster_centroids",
       "sc_cosine_distances_f64": "AgglomerativeClustering(cosine)",
       "sc_complete_linkage": "AgglomerativeClustering(cosine, complete)",
       "sc_average_linkage": "AgglomerativeClustering(cosine, average)",
@@ -252,22 +294,23 @@ class Engine:
     return nat.GEMM_SIMT if n < self.simt_below else nat.GEMM_TCGEN05
 
   def affinity(self, x_dev, want_crop_vector: bool):
-    """utils.compute_affinity_matrix on a device [n, d] fp32/fp64 tensor."""
+    """utils.compute_affinity_matrix on a device [n, d] fp16/bf16/fp32/fp64 tensor (row stride
+    free, unit column stride), read in place."""
     t = torch()
     n, d = int(x_dev.shape[0]), int(x_dev.shape[1])
     engine = self.gemm_engine(n)
     a = self.matrix(n)
     crop = self.vector(n, t.float32, zero=True) if want_crop_vector else None
-    is64 = 1 if x_dev.dtype == t.float64 else 0
+    code = dtype_code(x_dev)
     if engine == nat.GEMM_SIMT:
       xn = t.empty((n, round_up(d, 4)), dtype=t.float32, device=self.device)
-      self.call("sc_normalize_rows", _ptr(x_dev), is64, n, d, x_dev.stride(0), _ptr(xn),
+      self.call("sc_normalize_rows_typed", _ptr(x_dev), code, n, d, x_dev.stride(0), _ptr(xn),
                 xn.stride(0), None, None, 0, self.stream)
       self.call("sc_affinity_cosine", engine, self.gemm_precision, _ptr(xn), xn.stride(0), None,
                 None, 0, n, d, _ptr(a), a.stride(0), _ptr(crop), self.stream)
     else:
       hi, lo = self.planes(n, d)
-      self.call("sc_normalize_rows", _ptr(x_dev), is64, n, d, x_dev.stride(0), None, 0,
+      self.call("sc_normalize_rows_typed", _ptr(x_dev), code, n, d, x_dev.stride(0), None, 0,
                 _ptr(hi), _ptr(lo), hi.stride(0), self.stream)
       self.call("sc_affinity_cosine", engine, self.gemm_precision, None, 0, _ptr(hi), _ptr(lo),
                 hi.stride(0), n, d, _ptr(a), a.stride(0), _ptr(crop), self.stream)
@@ -441,12 +484,12 @@ class Engine:
 
   # ---- row panels of the factored route
   def normalized_planes(self, x_dev):
-    """Split fp16 planes of the row-normalised embeddings (the affinity GEMM's operands)."""
-    t = torch()
+    """Split fp16 planes of the row-normalised embeddings (the affinity GEMM's operands) of a
+    device [n, d] fp16/bf16/fp32/fp64 tensor."""
     n, d = int(x_dev.shape[0]), int(x_dev.shape[1])
     hi, lo = self.planes(n, d)
-    self.call("sc_normalize_rows", _ptr(x_dev), 1 if x_dev.dtype == t.float64 else 0, n, d,
-              x_dev.stride(0), None, 0, _ptr(hi), _ptr(lo), hi.stride(0), self.stream)
+    self.call("sc_normalize_rows_typed", _ptr(x_dev), dtype_code(x_dev), n, d, x_dev.stride(0),
+              None, 0, _ptr(hi), _ptr(lo), hi.stride(0), self.stream)
     return hi, lo
 
   def affinity_panel(self, hi, lo, n, d, a0, a1, crop=None):
@@ -618,6 +661,23 @@ class Engine:
     self.call("sc_cosine_distances_f64", _ptr(x_dev), 1 if x_dev.dtype == t.float64 else 0, n, d,
               x_dev.stride(0), _ptr(dist), dist.stride(0), _ptr(flag), self.stream)
     return dist, flag
+
+  def cluster_centroids(self, x_dev, labels: np.ndarray):
+    """utils.get_cluster_centroids bit for bit on a device [n, d] fp32/fp64 tensor and host labels
+    -> device fp64 [max(labels) + 1, d] (NaN rows for ids without a member)."""
+    t = torch()
+    labels = np.asarray(labels).astype(np.int64)
+    if labels.shape != (x_dev.shape[0],):
+      raise ValueError("labels must hold one id per embedding")
+    if labels.size and labels.min() < 0:
+      raise ValueError("'list' argument must have no negative elements")   # np.bincount's error
+    n, d = int(x_dev.shape[0]), int(x_dev.shape[1])
+    k = int(labels.max()) + 1
+    lab = t.from_numpy(labels).to(self.device)
+    out = t.empty((k, d), dtype=t.float64, device=self.device)
+    self.call("sc_cluster_centroids", _ptr(x_dev), 1 if x_dev.dtype == t.float64 else 0, n, d,
+              x_dev.stride(0), _ptr(lab), k, _ptr(out), out.stride(0), self.stream)
+    return out
 
   def complete_linkage(self, dist, n: int):
     """Complete-linkage NN-chain over the device distance matrix (overwritten) -> host

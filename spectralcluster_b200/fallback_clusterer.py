@@ -16,7 +16,9 @@ What runs where:
     launch that stops as soon as a second cluster opens (`sc_naive_cluster`); a host ndarray
     affinity still runs the host clusterer;
   * FallbackClusterer otherwise (inputs below `spectral_min_embeddings`,
-    FallbackClusterer.predict): host.
+    FallbackClusterer.predict): host for a host ndarray; a CUDA tensor stays on the device
+    (sc_naive_cluster for the Naive type, agglomerative.CosineAverageLinkage for the Agglomerative
+    type), with the labels the host call on its twin returns.
 """
 
 from __future__ import annotations
@@ -73,7 +75,17 @@ class FallbackClusterer:
     # any other value: the reference builds a ValueError without raising it (:121, SURVEY.md
     # A.4-4) and fails later with AttributeError in predict(); same here.
 
-  def predict(self, embeddings: np.ndarray) -> np.ndarray:
+  def predict(self, embeddings) -> np.ndarray:
+    """Labels of the rows of an ndarray, or of a CUDA tensor on the device: what the host call on
+    its twin (X.cpu().numpy(); for bfloat16, X.float().cpu().numpy()) returns."""
+    if naive_clusterer._is_cuda_tensor(embeddings):
+      from . import device as dev
+      x = dev.twin(embeddings.detach())
+      if self.options.fallback_clusterer_type == FallbackClustererType.Agglomerative:
+        from . import agglomerative
+        return agglomerative.CosineAverageLinkage(
+            self.options.agglomerative_threshold).fit_predict(x)
+      return self.clusterer.fit_predict(x)
     return self.clusterer.fit_predict(embeddings)
 
 
@@ -106,9 +118,9 @@ def check_single_cluster(fallback_options: FallbackOptions,
   For AffinityGmmBic on a device affinity, `details` (if given) receives the two BICs, both
   GMMs' EM iteration counts and the number of passes over the affinity.  Both fallback clusterer
   types on a device affinity run on the device too, on `embeddings_dev` (the embeddings as a CUDA
-  tensor) when given and on an uploaded copy of `embeddings` otherwise; the Naive type stops at
-  the second cluster and records the embeddings it processed and the clusters it opened in
-  `details`."""
+  tensor, read as its host twin's dtype: fp16 as fp64, bf16 as fp32) when given and on an uploaded
+  copy of `embeddings` otherwise; the Naive type stops at the second cluster and records the
+  embeddings it processed and the clusters it opened in `details`."""
   cond = fallback_options.single_cluster_condition
   thr = fallback_options.single_cluster_affinity_threshold
   if cond == SingleClusterCondition.AllAffinity:
@@ -138,15 +150,16 @@ def check_single_cluster(fallback_options: FallbackOptions,
     kind = fallback_options.fallback_clusterer_type
     if kind == FallbackClustererType.Agglomerative and not isinstance(affinity, np.ndarray):
       from . import agglomerative
+      from . import device as dev
       probe = agglomerative.CosineAverageLinkage(fallback_options.agglomerative_threshold)
-      probe.fit_predict(embeddings if embeddings_dev is None else embeddings_dev)
+      probe.fit_predict(embeddings if embeddings_dev is None else dev.twin(embeddings_dev))
       return probe.n_clusters_ == 1
     if kind == FallbackClustererType.Naive and not isinstance(affinity, np.ndarray):
       from . import device as dev
       probe = naive_clusterer.NaiveClusterer(fallback_options.naive_threshold,
                                              fallback_options.naive_adaptation_threshold)
       eng = dev.Engine.get()
-      x = embeddings_dev
+      x = None if embeddings_dev is None else dev.twin(embeddings_dev)
       if x is None:
         x = np.ascontiguousarray(embeddings)
         if x.dtype not in (np.float32, np.float64):

@@ -2,7 +2,8 @@
 (/root/reference/spectralcluster/spectral_clusterer.py: __init__ :29-106,
 _compute_eigenvectors_ncluster :108-168, predict :201-314) whose arithmetic runs on an H100.
 
-predict(): one H2D copy of the [N, d] embeddings, every N x N intermediate stays in HBM
+predict(): one H2D copy of the [N, d] embeddings (none when they come as a CUDA tensor, which is
+read in place as its host twin would be), every N x N intermediate stays in HBM
 (affinity GEMM -> fused refinement -> Diffuse GEMM -> row statistics -> symmetric eigensolve ->
 k-means), one D2H copy of N labels.  The callers around the path follow the reference: the
 fallback clusterer for tiny inputs is host code (scikit-learn, as in the reference); the
@@ -26,6 +27,7 @@ from . import device as dev
 from . import eigen_windows
 from . import fallback_clusterer
 from . import laplacian as laplacian_lib
+from . import naive_clusterer
 from . import refinement
 from . import utils
 
@@ -281,19 +283,31 @@ class SpectralClusterer:
     _, v, k, gap = self._eigen_on_device(eng, da, constraint_matrix)
     return v.to("cpu").numpy(), k, gap
 
-  def _reduce_size_and_predict(self, embeddings: np.ndarray) -> np.ndarray:
+  def _reduce_size_and_predict(self, embeddings) -> np.ndarray:
     """spectral_clusterer.py:170-199: complete-linkage cosine AHC down to `max_spectral_size`
     clusters (the reference's own lossy answer to large N, on the device with scikit-learn's labels
     -- see agglomerative.py; BASELINE configs[3] shards the exact problem instead), spectral
-    clustering of the cluster centroids on the device, labels chained back."""
-    pre = agglomerative.CosineCompleteLinkage(
-        n_clusters=self.max_spectral_size).fit_predict(embeddings)
-    centroids = utils.get_cluster_centroids(embeddings, pre)
+    clustering of the cluster centroids on the device, labels chained back.  A CUDA tensor stays on
+    the device: its centroids are a device fp64 tensor (sc_cluster_centroids), clustered in turn."""
+    on_device = not isinstance(embeddings, np.ndarray)
+    x = dev.twin(embeddings) if on_device else embeddings
+    pre = agglomerative.CosineCompleteLinkage(n_clusters=self.max_spectral_size).fit_predict(x)
+    if on_device:
+      centroids = dev.Engine.get().cluster_centroids(x, pre)
+    else:
+      centroids = utils.get_cluster_centroids(embeddings, pre)
     return utils.chain_labels(pre, self.predict(centroids))
 
   # ------------------------------------------------------------------ predict
-  def predict(self, embeddings: np.ndarray, constraint_matrix=None) -> np.ndarray:
-    """Cluster the rows of `embeddings` ([n_samples, n_features] ndarray) -> int64 labels."""
+  def predict(self, embeddings, constraint_matrix=None) -> np.ndarray:
+    """Cluster the rows of `embeddings` -> int64 labels (a host ndarray).
+
+    `embeddings` is an [n_samples, n_features] ndarray, or a CUDA tensor on the device
+    Engine.get() serves (float16, bfloat16, float32 or float64; integer and bool tensors are
+    widened to float64; any row stride).  A CUDA tensor X is clustered in place, never copied to
+    the host except where a user `affinity_function` or scikit-learn must receive an ndarray, and
+    gives what its host twin gives, bit for bit: X.cpu().numpy(), or X.float().cpu().numpy() for
+    bfloat16."""
     if self.collect_timings and dev.torch().cuda.is_available():
       eng = dev.Engine.get()
       if eng.profile is None:
@@ -304,14 +318,21 @@ class SpectralClusterer:
           self.last_timings = eng.stop_profile()
     return self._predict(embeddings, constraint_matrix)
 
-  def _predict(self, embeddings: np.ndarray, constraint_matrix=None) -> np.ndarray:
+  def _predict(self, embeddings, constraint_matrix=None) -> np.ndarray:
     num_embeddings = embeddings.shape[0]
-    if not isinstance(embeddings, np.ndarray):
+    on_device = naive_clusterer._is_cuda_tensor(embeddings)
+    if not on_device and not isinstance(embeddings, np.ndarray):
       raise TypeError("embeddings must be a numpy array")
     if len(embeddings.shape) != 2:
       raise ValueError("embeddings must be 2-dimensional")
+    if on_device:
+      serves = dev.torch().cuda.current_device()
+      if embeddings.device.index != serves:
+        raise ValueError("embeddings are on %s, but predict() runs on cuda:%d (the current device)"
+                         % (embeddings.device, serves))
+      given, embeddings = embeddings, dev.device_embeddings(embeddings)
     if num_embeddings < self.fallback_options.spectral_min_embeddings:
-      # too few embeddings for a spectrum (spectral_clusterer.py:230-234): host fallback clusterer
+      # too few embeddings for a spectrum (spectral_clusterer.py:230-234): the fallback clusterer
       return fallback_clusterer.FallbackClusterer(self.fallback_options).predict(embeddings)
     if self.max_spectral_size is not None and num_embeddings > self.max_spectral_size:
       if constraint_matrix is not None:
@@ -324,30 +345,33 @@ class SpectralClusterer:
     eng = dev.Engine.get()
     t = dev.torch()
     sequence = list(self.refinement_options.refinement_sequence or [])
+    builtin = self.affinity_function is utils.compute_affinity_matrix
+    if builtin and on_device:
+      x_dev = embeddings
+    elif builtin:
+      x = np.ascontiguousarray(embeddings)
+      if x.dtype not in (np.float32, np.float64):
+        x = x.astype(np.float64)
+      x_dev = t.from_numpy(x).to(eng.device, non_blocking=True)
     if self._factored_route(eng, num_embeddings, constraint_matrix):
-      x = np.ascontiguousarray(embeddings)
-      if x.dtype not in (np.float32, np.float64):
-        x = x.astype(np.float64)
-      x_dev = t.from_numpy(x).to(eng.device, non_blocking=True)
       affinity = dev.FactoredAffinity(eng, x_dev)
-    elif self.affinity_function is utils.compute_affinity_matrix:
-      x = np.ascontiguousarray(embeddings)
-      if x.dtype not in (np.float32, np.float64):
-        x = x.astype(np.float64)
-      x_dev = t.from_numpy(x).to(eng.device, non_blocking=True)
+    elif builtin:
       crop_first = bool(sequence) and sequence[0] == RefinementName.CropDiagonal
       a, crop = eng.affinity(x_dev, want_crop_vector=crop_first)
       affinity = DeviceAffinity(a, num_embeddings, crop, True)
     else:
-      x_dev = None
-      host = np.asarray(self.affinity_function(embeddings))
+      # the reference hands the user's function an ndarray: a CUDA tensor's host twin
+      x_dev = dev.twin(embeddings) if on_device else None
+      host = np.asarray(self.affinity_function(
+          dev.host_twin(given) if on_device else embeddings))
       affinity = DeviceAffinity(eng.upload_matrix(host), num_embeddings, None,
                                 bool(np.allclose(host, host.T, rtol=1e-6, atol=1e-9)))
 
     single_details = {}
     if self.min_clusters == 1:
       # single-vs-multi cluster decision on the resident affinity (spectral_clusterer.py:253-256)
-      if fallback_clusterer.check_single_cluster(self.fallback_options, embeddings, affinity,
+      if fallback_clusterer.check_single_cluster(self.fallback_options,
+                                                 None if on_device else embeddings, affinity,
                                                  single_details, embeddings_dev=x_dev):
         if single_details:
           self.last_details = dict(single_cluster=single_details)
