@@ -444,6 +444,17 @@ int sc_eigh_extremal_factored(sc_context* ctx, const void* y_hi, int64_t n, int6
                               double tol, int64_t max_matvecs, double* w_host, double* v_dev,
                               int64_t* stats_host, void* stream);
 
+/* One window of a windowed solve on the factored operator: sc_eigh_extremal_locked with `y_hi` /
+ * `ldy` (as in sc_eigh_extremal_factored) in place of `s` / `lds`.  Finds the next n_values
+ * extremal eigenvalues of M on the complement of locked[0..n_locked) and appends their
+ * symmetrised-space Ritz vectors at locked[n_locked..).  SYNCHRONOUS. */
+int sc_eigh_extremal_locked_factored(sc_context* ctx, const void* y_hi, int64_t n, int64_t ldy,
+                                     const double* delta, const double* left, const double* right,
+                                     double sign, int which, int64_t n_values, double tol,
+                                     int64_t max_matvecs, double scale, double* locked,
+                                     int64_t n_locked, double* w_host, int64_t* stats_host,
+                                     void* stream);
+
 /* ---- Krylov primitives of the general (non-symmetrisable) eigen path: utils.py:59-61 is
  * np.linalg.eig + .real; sequences such as [RowWiseThreshold] alone leave a genuinely
  * non-symmetric matrix (SURVEY.md 8(f)-1).  The Krylov-Schur recurrence is host logic

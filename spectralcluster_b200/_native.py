@@ -110,6 +110,9 @@ PROTOTYPES = {
                              c_i64, c_ptr],
     "sc_eigh_extremal_factored": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_dbl, c_int,
                                   c_i64, c_i64, c_dbl, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_eigh_extremal_locked_factored": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_dbl,
+                                         c_int, c_i64, c_dbl, c_i64, c_dbl, c_ptr, c_i64, c_ptr,
+                                         c_ptr, c_ptr],
     "sc_affinity_cosine_panel": [c_ptr, c_int, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64,
                                  c_ptr, c_i64, c_ptr, c_ptr],
     "sc_blur_upper_rowmax_block": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr,

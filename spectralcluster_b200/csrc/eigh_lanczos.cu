@@ -1201,6 +1201,24 @@ extern "C" int sc_eigh_extremal_locked(sc_context* ctx, const float* s, int64_t 
                       nullptr, stats_host, stream);
 }
 
+// One window of the windowed solve on the factored operator S = Y Y^T (S never formed).  The
+// scratch of lanczos_impl holds both at once: `mid` (the Y T intermediate) sits after `wb` in
+// `work` and is touched only by the block product, while the locked-set deflation uses `partial`
+// (sized for LOCK_CHUNK rows) and `lock_small`, neither of which the block product reads.
+extern "C" int sc_eigh_extremal_locked_factored(sc_context* ctx, const void* y_hi, int64_t n,
+                                                int64_t ldy, const double* delta,
+                                                const double* left, const double* right,
+                                                double sign, int which, int64_t n_values,
+                                                double tol, int64_t max_matvecs, double scale,
+                                                double* locked, int64_t n_locked, double* w_host,
+                                                int64_t* stats_host, void* stream) {
+  SC_REQUIRE(y_hi, "sc_eigh_extremal_locked_factored: y_hi missing");
+  SC_REQUIRE(locked, "sc_eigh_extremal_locked_factored: locked buffer missing");
+  return lanczos_impl(ctx, nullptr, (const __half*)y_hi, n, 0, n, ldy, delta, left, right, sign,
+                      which, n_values, 0, tol, max_matvecs, nullptr, 0, 0, nullptr, nullptr, locked,
+                      n_locked, scale, w_host, nullptr, stats_host, stream);
+}
+
 extern "C" int sc_eigh_mapback(sc_context* ctx, const double* u, int64_t n, const int* cols_host,
                                int64_t k, const double* left, const double* right, double* v_out,
                                void* stream) {

@@ -241,6 +241,7 @@ class Engine:
       "sc_eigh_extremal_sharded": "utils.compute_sorted_eigenvectors",
       "sc_eigh_extremal_locked": "utils.compute_sorted_eigenvectors",
       "sc_eigh_extremal_locked_sharded": "utils.compute_sorted_eigenvectors",
+      "sc_eigh_extremal_locked_factored": "utils.compute_sorted_eigenvectors",
       "sc_eigh_mapback": "utils.compute_sorted_eigenvectors",
       "sc_kmeans": "custom_distance_kmeans.run_kmeans", "sc_row_renorm": "spectral_clusterer.row_wise_renorm",
       "sc_affinity_stats": "fallback_clusterer.check_single_cluster",
@@ -571,11 +572,15 @@ class Engine:
   def eigh_window(self, s, n, delta, left, right, sign, which, n_values, locked, n_locked, scale,
                   tol=1e-9, max_matvecs=0):
     """The next n_values extremal eigenvalues (host fp64) on the complement of locked[:n_locked]
-    (device fp64 [capacity, n]); their symmetrised-space vectors land in locked[n_locked:]."""
+    (device fp64 [capacity, n]); their symmetrised-space vectors land in locked[n_locked:].  The
+    operand decides the operator: an fp32 `s` is S itself, an fp16 `s` is Y_hi of the factored
+    operator S = Y_hi Y_hi^T (sc_eigh_extremal_locked_factored), never formed."""
     w = np.empty(n_values, dtype=np.float64)
     stats = np.zeros(4, dtype=np.int64)
     assert locked.shape[0] >= n_locked + n_values and locked.shape[1] == n and locked.is_contiguous()
-    self.call("sc_eigh_extremal_locked", _ptr(s), n, s.stride(0), _ptr(delta), _ptr(left),
+    entry = ("sc_eigh_extremal_locked_factored" if s.dtype == torch().float16
+             else "sc_eigh_extremal_locked")
+    self.call(entry, _ptr(s), n, s.stride(0), _ptr(delta), _ptr(left),
               _ptr(right), float(sign), int(which), n_values, float(tol), int(max_matvecs),
               float(scale), _ptr(locked), n_locked, w.ctypes.data_as(ctypes.c_void_p),
               stats.ctypes.data_as(ctypes.c_void_p), self.stream)

@@ -15,7 +15,8 @@ max_clusters is None, but only a prefix of it can change its answer:
 
 Such a prefix is "settled".  `solve` grows the prefix a window of WINDOW_PAIRS eigenpairs at a
 time until it is: on the device each window is a block Lanczos solve on the complement of the
-pairs already found (sc_eigh_extremal_locked), on the CPU a NumPy backend stands in (tests).
+pairs already found (sc_eigh_extremal_locked, or sc_eigh_extremal_locked_factored on the factored
+operator), on the CPU a NumPy backend stands in (tests).
 `grow_krylov_schur` applies the same rule to the general (non-symmetrisable) path, whose
 Krylov-Schur solver is restarted with twice the pairs until the prefix settles.
 """
@@ -161,13 +162,18 @@ class NumpyOps:
 
 class DeviceOps:
   """Windows on the device: sc_eigh_extremal_locked on the implicit operator
-  diag(delta) + sign * diag(left) S diag(right), its Ritz vectors kept in HBM."""
+  diag(delta) + sign * diag(left) S diag(right), its Ritz vectors kept in HBM.  `factored`: `s` is
+  the fp16 Y_hi of S = Y_hi Y_hi^T, never formed, and the windows and the lambda_max solve run on
+  the factored operator (sc_eigh_extremal_locked_factored, sc_eigh_extremal_factored)."""
 
-  def __init__(self, eng, s, n, delta, left, right, sign, which, capacity):
+  def __init__(self, eng, s, n, delta, left, right, sign, which, capacity, factored=False):
     from . import device as dev
     from . import _native as nat
     t = dev.torch()
     self.eng, self.op, self.which, self.largest = eng, (s, n, delta, left, right, sign), which, nat.EIG_LARGEST
+    # Engine.eigh_window picks the locked entry from the operand's dtype (fp16: Y_hi)
+    assert not factored or s.dtype == t.float16
+    self.factored = factored
     self.locked = t.empty((capacity, n), dtype=t.float64, device=eng.device)
     self.count, self.scale = 0, 0.0
     self.stats = dict(windows=0, passes=0, matvecs=0, restarts=0)
@@ -183,7 +189,10 @@ class DeviceOps:
     return w
 
   def lambda_max(self):
-    w, _, st = self.eng.eigh(*self.op, self.largest, 1, 0, False)
+    if self.factored:
+      w, _, st = self.eng.eigh_factored(*self.op, self.largest, 1, 0)
+    else:
+      w, _, st = self.eng.eigh(*self.op, self.largest, 1, 0, False)
     self.scale = max(self.scale, abs(float(w[0])))
     self.stats["passes"] += int(st[3])
     return float(w[0])

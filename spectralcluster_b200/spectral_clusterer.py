@@ -171,8 +171,8 @@ class SpectralClusterer:
       else:
         w, v, stats = arnoldi.eig_extremal_device(eng, *op, not descend, limit, n_vectors)
         top_solve = lambda: arnoldi.eig_extremal_device(eng, *op, False, 1, 0)[0]
-    elif refined.y_hi is not None:
-      # factored operator (the scope of both routes guarantees lanczos_fits): S = Y_hi Y_hi^T is
+    elif refined.y_hi is not None and lanczos_fits(n, limit):
+      # factored operator, one solve (the bounded route and _factored_route): S = Y_hi Y_hi^T is
       # never stored.  `solver` names the route's choice: one Lanczos solve after the bounded
       # Diffuse of the stored front end, "lanczos-factored" on the panel route.
       solver = "lanczos" if refined.tiles is not None else "lanczos-factored"
@@ -185,12 +185,17 @@ class SpectralClusterer:
       w, v, stats = eng.eigh(*op, which, limit, n_vectors, False)
       stats = stats.tolist()
       top_solve = lambda: eng.eigh(*op, nat.EIG_LARGEST, 1, 0, False)[0]
-    elif n > DENSE_MAX_N:
+    elif n > DENSE_MAX_N or refined.y_hi is not None:
       # more pairs than one Lanczos solve finds, above the dense solver's n: windows of block
-      # Lanczos on the complement of the pairs found, until the eigengap is decided
-      solver, top_solve = "lanczos-windows", None
-      ops = eigen_windows.DeviceOps(eng, *op, which, capacity=eigen_windows.capacity(
-          n, self.max_clusters, self.min_clusters))
+      # Lanczos on the complement of the pairs found, until the eigengap is decided; on the
+      # stored S, or on the factored operator of _factored_windows_route
+      factored = refined.y_hi is not None
+      solver = "lanczos-factored-windows" if factored else "lanczos-windows"
+      top_solve = None
+      ops = eigen_windows.DeviceOps(eng, *((refined.y_hi,) + op[1:] if factored else op), which,
+                                    capacity=eigen_windows.capacity(
+                                        n, self.max_clusters, self.min_clusters),
+                                    factored=factored)
       prefix = eigen_windows.solve(ops, descend, self.max_clusters, self.min_clusters,
                                    self.stop_eigenvalue, self.eigengap_type, n=n)
       w, top = prefix.values[:limit], prefix.lambda_max
@@ -225,32 +230,47 @@ class SpectralClusterer:
       self.last_details["diffuse"] = dict(tiles=computed, of=total, operator="factored")
     return w, v, k, gap
 
-  def _lanczos_scope(self, eng, n: int, constraint_matrix=None) -> bool:
-    """The options both routes that never store S serve: the default affinity, the fused chain
-    closed by a single-MMA Diffuse (dev.factored_sequence_ok), no constraint, and one Lanczos solve
-    (bounded max_clusters < LANCZOS_MAX_PAIRS that lanczos_fits)."""
-    limit = (self.max_clusters or 0) + 1
+  def _operator_scope(self, eng, n: int, constraint_matrix=None) -> bool:
+    """The options every route that never stores S serves: the default affinity, the fused chain
+    closed by a single-MMA Diffuse (dev.factored_sequence_ok), no constraint, min_clusters != 1 and
+    no autotune_group."""
     return (self.affinity_function is utils.compute_affinity_matrix and
-            self.min_clusters != 1 and (self.min_clusters or 0) <= limit and
+            self.min_clusters != 1 and
             not (self.constraint_options and constraint_matrix is not None) and
-            self.max_clusters is not None and self.max_clusters < LANCZOS_MAX_PAIRS and
             self.autotune_group is None and
             dev.factored_sequence_ok(eng, self.refinement_options) and
-            n > limit and n > eng.dense_eig_max and lanczos_fits(n, limit) and
             eng.gemm_engine(n) == nat.GEMM_TCGEN05 and
             eng.diffuse_precision_for(n) == nat.GEMM_SINGLE)
 
+  def _lanczos_scope(self, eng, n: int, constraint_matrix=None) -> bool:
+    """The calls of _operator_scope that one Lanczos solve serves (bounded max_clusters <
+    LANCZOS_MAX_PAIRS that lanczos_fits): those of the two one-solve routes below."""
+    limit = (self.max_clusters or 0) + 1
+    return (self.max_clusters is not None and self.max_clusters < LANCZOS_MAX_PAIRS and
+            (self.min_clusters or 0) <= limit and
+            n > limit and n > eng.dense_eig_max and lanczos_fits(n, limit) and
+            self._operator_scope(eng, n, constraint_matrix))
+
   def _factored_route(self, eng, n: int, constraint_matrix=None) -> bool:
-    """Whether predict() on n embeddings takes the factored route: the stored route's peak
-    (computed from shapes) exceeds eng.factored_above_bytes and every option is one the factored
-    route serves; any other call keeps the stored route."""
+    """Whether predict() on n embeddings takes the factored route with one Lanczos solve: the
+    stored route's peak (computed from shapes) exceeds eng.factored_above_bytes and every option
+    is one _lanczos_scope accepts.  _factored_windows_route covers the eigen options one solve
+    cannot serve; any other call keeps the stored route."""
     return (self._lanczos_scope(eng, n, constraint_matrix) and
             dev.stored_route_peak_bytes(n) > eng.factored_above_bytes)
 
+  def _factored_windows_route(self, eng, n: int, constraint_matrix=None) -> bool:
+    """Whether predict() on n embeddings takes the factored route with the windowed solve
+    (eigen_windows.py on the factored operator): as _factored_route, but for max_clusters=None or
+    more pairs than one Lanczos solve finds.  Disjoint from _factored_route."""
+    return ((self.max_clusters is None or self.max_clusters + 1 > LANCZOS_MAX_PAIRS) and
+            n > DENSE_MAX_N and dev.stored_route_peak_bytes(n) > eng.factored_above_bytes and
+            self._operator_scope(eng, n, constraint_matrix))
+
   def _bounded_route(self, eng, n: int, constraint_matrix=None) -> bool:
     """Whether the stored front end (a resident affinity) replaces the storing Diffuse and the
-    stored Lanczos solve by the bounded Diffuse and a Lanczos solve on the factored operator: the
-    calls of _lanczos_scope from N = dev.BOUNDED_FROM that do not take the factored route."""
+    stored Lanczos solve by the bounded Diffuse and one Lanczos solve on the factored operator:
+    the calls of _lanczos_scope from N = dev.BOUNDED_FROM that do not take the factored route."""
     return (n >= dev.BOUNDED_FROM and self._lanczos_scope(eng, n, constraint_matrix) and
             dev.stored_route_peak_bytes(n) <= eng.factored_above_bytes)
 
@@ -353,7 +373,8 @@ class SpectralClusterer:
       if x.dtype not in (np.float32, np.float64):
         x = x.astype(np.float64)
       x_dev = t.from_numpy(x).to(eng.device, non_blocking=True)
-    if self._factored_route(eng, num_embeddings, constraint_matrix):
+    if (self._factored_route(eng, num_embeddings, constraint_matrix) or
+        self._factored_windows_route(eng, num_embeddings, constraint_matrix)):
       affinity = dev.FactoredAffinity(eng, x_dev)
     elif builtin:
       crop_first = bool(sequence) and sequence[0] == RefinementName.CropDiagonal
