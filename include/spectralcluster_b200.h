@@ -188,6 +188,13 @@ int sc_diffuse_tile_list(sc_context* ctx, const float* norms, int64_t groups, co
 int sc_diffuse_rowmax_tiles(sc_context* ctx, const void* yp_hi, int64_t ldh, int64_t n,
                             const uint32_t* tiles, const int* count, const int* perm,
                             float* rowmax, void* stream);
+/* sc_bound_order: the row order of the bounded Diffuse from the group-norm profiles norms [n, groups]
+ * (those of sc_row_group_bounds): spherical k-means with k <= 16 centres (greedy farthest-point
+ * seeds from row 0, `passes` assignments) and a stable sort by label; perm (device int32 [n])
+ * receives the rows in that order.  Deterministic, and enqueued only (no host synchronisation).
+ * Profiles that are all alike give the natural order. */
+int sc_bound_order(sc_context* ctx, const float* norms, int64_t n, int64_t groups, int k, int passes,
+                   int* perm, void* stream);
 
 /* Row maxima and row sums (fp64) of an fp32 matrix: the reductions of
  * RowWiseNormalize (refinement.py:243) and of the degree (laplacian.py:41). */

@@ -58,6 +58,7 @@ PROTOTYPES = {
     "sc_gather_rows_f16": [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr],
     "sc_diffuse_tile_list": [c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_diffuse_rowmax_tiles": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_bound_order": [c_ptr, c_ptr, c_i64, c_i64, c_int, c_int, c_ptr, c_ptr],
     "sc_row_stats": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     "sc_affinity_stats": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr],
     "sc_row_normalize": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr],

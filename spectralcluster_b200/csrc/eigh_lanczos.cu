@@ -14,6 +14,7 @@
 //                   the fp64 tensor cores.  A block of b >= (number of wanted pairs) vectors also
 //                   makes the solver find every copy of a repeated eigenvalue (a single start
 //                   vector with full re-orthogonalisation can only ever see one).
+//                   k_symm_dmma_f16 is the same product on an fp16 matrix (the factored operator).
 //   k_block_proj / k_block_axpy   block classical Gram-Schmidt (twice) of the b products against
 //                   the N x m basis, then Cholesky-QR (twice) inside the block
 //   k_proj / k_axpy_basis   the same one vector at a time, for a rank-deficient block
@@ -35,6 +36,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <numeric>
+#include <type_traits>
 #include <vector>
 
 namespace sc {
@@ -91,13 +93,8 @@ constexpr int SYMM_ROWS = 256, SYMM_COLS = 32, SYMM_SP = 36, SYMM_TP = 36, SYMM_
 constexpr int SYMM_S_FLOATS = SYMM_ROWS * SYMM_SP;                       // 9,216 floats = 36,864 B
 constexpr int SYMM_STAGE_BYTES = SYMM_S_FLOATS * 4 + SYMM_MAXB * SYMM_TP * 8;   // + 4,608 B
 constexpr int SYMM_STAGES = 2;     // x 41,472 B: two CTAs (16 warps) per SM
-// The factored operator (sc_eigh_extremal_factored) stages an fp16 matrix in the same stage
-// buffers: 256 rows x 32 columns of fp16 at a row pitch of 40 halves (80 B: 16-byte aligned rows,
-// and the eight rows of an A fragment land on distinct bank quads).  fp16 -> fp64 is exact.
 template <typename T> struct SymmElem;
 template <> struct SymmElem<float> { static constexpr int SP = SYMM_SP; };
-template <> struct SymmElem<__half> { static constexpr int SP = 40; };
-static_assert(SYMM_ROWS * 40 * 2 <= SYMM_S_FLOATS * 4, "fp16 tile fits the fp32 stage");
 
 __device__ __forceinline__ double to_f64(float x) { return (double)x; }
 __device__ __forceinline__ double to_f64(__half x) { return (double)__half2float(x); }
@@ -203,6 +200,122 @@ k_symm_dmma(const T* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
   }
 }
 
+// The same block product on an fp16 matrix (the factored operator Y (Y T) of
+// sc_eigh_extremal_factored, its windows and the row sums of the bounded Diffuse), with the same
+// work items, column splits and k order, so every output is bit for bit what k_symm_dmma gives on
+// the fp32 upcast (fp16 -> fp64 is exact).  Two things differ from the fp32 kernel:
+//   stage = 256 rows x 64 columns of fp16 (128 B per row: whole L2 lines; a 64 B half line per row
+//           and stage streams at about 1.95 TB/s, a 128 B line at 3.05 TB/s on the H100) at a row
+//           pitch of 72 halves (144 B: 16-byte aligned rows, and the eight rows of an A fragment
+//           land on distinct bank quads), + b vectors x 64 columns of T at a pitch of 68 doubles;
+//   MMA   = mma.sync.m16n8k4.f64: the two m8n8k4 steps of row groups g and g + 1 on the same four
+//           columns in one instruction.  Issued as separate m8n8k4 steps, the MMAs alone (stages
+//           loaded once and reused, no HBM traffic) take ~4.4 ms per pass over a 65,536^2 fp16
+//           matrix at any b, well above the 2.6 ms HBM floor; paired they take 2.3-2.45 ms.
+constexpr int SYMH_COLS = 64, SYMH_SP = 72, SYMH_TP = 68;
+constexpr int SYMH_S_BYTES = SYMM_ROWS * SYMH_SP * 2;                       // 36,864 B
+constexpr int SYMH_STAGE_BYTES = SYMH_S_BYTES + SYMM_MAXB * SYMH_TP * 8;    // + 8,704 B
+constexpr int SYMH_STAGES = 2;     // x 45,568 B: two CTAs (16 warps) per SM
+
+__global__ void __launch_bounds__(256, 2)
+k_symm_dmma_f16(const __half* __restrict__ s, int64_t rows, int64_t n, int64_t lds,
+                const double* __restrict__ t /*[b][ldt]*/, int64_t ldt, int b, int row_blocks,
+                int64_t cols_per_split, double* __restrict__ partial /*[split][b][rows_pad]*/,
+                int64_t rows_pad) {
+  extern __shared__ __align__(16) unsigned char symm_smem[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int rb = blockIdx.x % row_blocks, split = blockIdx.x / row_blocks;
+  const int64_t row0 = (int64_t)rb * SYMM_ROWS;
+  const int64_t c_begin = (int64_t)split * cols_per_split;
+  const int64_t c_end = min(n, c_begin + cols_per_split);
+  const int chunks = (int)((c_end - c_begin + SYMH_COLS - 1) / SYMH_COLS);
+  auto stage_s = [&](int st) { return reinterpret_cast<__half*>(symm_smem + (size_t)st * SYMH_STAGE_BYTES); };
+  auto stage_t = [&](int st) {
+    return reinterpret_cast<double*>(symm_smem + (size_t)st * SYMH_STAGE_BYTES + SYMH_S_BYTES);
+  };
+  // fill: 256 rows x 8 16-byte granules of S, 8 per thread; b rows x 32 granules of T.  Past c_end
+  // both are zero-filled: the extra k steps at the end of a split add exact zeros.
+  auto fill = [&](int ch, int st) {
+    const int64_t c0 = c_begin + (int64_t)ch * SYMH_COLS;
+    __half* ss = stage_s(st);
+#pragma unroll
+    for (int k = 0; k < SYMM_ROWS * (SYMH_COLS / 8) / 256; ++k) {
+      const int idx = threadIdx.x + k * 256;
+      const int r = idx / (SYMH_COLS / 8), q = idx % (SYMH_COLS / 8);
+      const int64_t gr = (row0 + r < rows) ? row0 + r : rows - 1;
+      const int64_t gc = c0 + 8 * q;
+      int64_t valid = c_end - gc;
+      valid = valid < 0 ? 0 : (valid > 8 ? 8 : valid);
+      cp_async16_zfill(ss + r * SYMH_SP + 8 * q, s + gr * lds + (valid > 0 ? gc : 0), (int)valid * 2);
+    }
+    double* ts = stage_t(st);
+    for (int idx = threadIdx.x; idx < b * (SYMH_COLS / 2); idx += 256) {
+      const int p = idx / (SYMH_COLS / 2), q = idx % (SYMH_COLS / 2);
+      const int64_t gc = c0 + 2 * q;
+      int64_t valid = c_end - gc;
+      valid = valid < 0 ? 0 : (valid > 2 ? 2 : valid);
+      cp_async16_zfill(ts + p * SYMH_TP + 2 * q, t + (int64_t)p * ldt + (valid > 0 ? gc : 0), (int)valid * 8);
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  double acc[4][2][2];
+#pragma unroll
+  for (int g = 0; g < 4; ++g)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) acc[g][h][0] = acc[g][h][1] = 0.0;
+  const int fr = lane >> 2, fk = lane & 3;
+  const bool n1_live = (8 + fr) < b;                    // second n-tile: vectors 8..15
+  const bool n0_live = fr < b;
+  const bool two_tiles = b > 8;                         // block-uniform
+#pragma unroll
+  for (int st = 0; st < SYMH_STAGES - 1; ++st) {
+    if (st < chunks) fill(st, st);
+    else asm volatile("cp.async.commit_group;" ::: "memory");
+  }
+  for (int ch = 0; ch < chunks; ++ch) {
+    asm volatile("cp.async.wait_group %0;" ::"n"(SYMH_STAGES - 2) : "memory");
+    __syncthreads();                                    // chunk ch landed; stage (ch-1)%S is free
+    if (ch + SYMH_STAGES - 1 < chunks) fill(ch + SYMH_STAGES - 1, (ch + SYMH_STAGES - 1) % SYMH_STAGES);
+    else asm volatile("cp.async.commit_group;" ::: "memory");
+    const __half* ss = stage_s(ch % SYMH_STAGES) + (warp * 32 + fr) * SYMH_SP + fk;
+    const double* ts = stage_t(ch % SYMH_STAGES) + fk;
+#pragma unroll
+    for (int ks = 0; ks < SYMH_COLS / 4; ++ks) {
+      const double b0 = n0_live ? ts[fr * SYMH_TP + 4 * ks] : 0.0;
+      const double b1 = n1_live ? ts[(8 + fr) * SYMH_TP + 4 * ks] : 0.0;
+#pragma unroll
+      for (int g = 0; g < 4; g += 2) {
+        // A fragment of m16n8k4: rows fr (group g) and 8 + fr (group g + 1), column fk
+        const double a0 = to_f64(ss[g * 8 * SYMH_SP + 4 * ks]);
+        const double a1 = to_f64(ss[(g + 1) * 8 * SYMH_SP + 4 * ks]);
+        asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0, %1, %2, %3}, {%4, %5}, {%6}, "
+                     "{%0, %1, %2, %3};"
+                     : "+d"(acc[g][0][0]), "+d"(acc[g][0][1]), "+d"(acc[g + 1][0][0]), "+d"(acc[g + 1][0][1])
+                     : "d"(a0), "d"(a1), "d"(b0));
+        if (two_tiles)                                  // b <= 8: the second n-tile would be all zeros
+          asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0, %1, %2, %3}, {%4, %5}, {%6}, "
+                       "{%0, %1, %2, %3};"
+                       : "+d"(acc[g][1][0]), "+d"(acc[g][1][1]), "+d"(acc[g + 1][1][0]), "+d"(acc[g + 1][1][1])
+                       : "d"(a0), "d"(a1), "d"(b1));
+      }
+    }
+  }
+  // C fragment: row = fr of the group, vectors 8 h + 2 fk + {0, 1} (that of m8n8k4 per group)
+  double* out = partial + (int64_t)split * b * rows_pad;
+#pragma unroll
+  for (int g = 0; g < 4; ++g) {
+    const int64_t row = row0 + warp * 32 + g * 8 + fr;
+    if (row >= rows) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int p = 8 * h + 2 * fk + e;
+        if (p < b) out[(int64_t)p * rows_pad + row] = acc[g][h][e];
+      }
+  }
+}
+
 // y[p][row] = sum over the column splits, in order
 __global__ void k_symm_reduce(const double* __restrict__ partial, int splits, int b, int64_t rows,
                               int64_t rows_pad, double* __restrict__ y, int64_t ldy) {
@@ -231,7 +344,7 @@ static size_t block_product_scratch_doubles(int64_t rows, int64_t n, int b, int 
   return (size_t)splits * b * rows_pad;
 }
 
-// Y = S T (k_symm_dmma, then k_symm_reduce); `scratch`, `splits` and `cols_per_split` come from
+// Y = S T (k_symm_dmma or, for fp16, k_symm_dmma_f16, then k_symm_reduce); `scratch`, `splits` and `cols_per_split` come from
 // block_product_scratch_doubles
 template <typename T>
 static int launch_block_product(int b, const T* s, int64_t rows, int64_t n, int64_t lds,
@@ -242,10 +355,17 @@ static int launch_block_product(int b, const T* s, int64_t rows, int64_t n, int6
              "sc_eigh_extremal: internal (block product alignment)");
   const int row_blocks = (int)((rows + SYMM_ROWS - 1) / SYMM_ROWS);
   const int64_t rows_pad = (rows + 1) & ~(int64_t)1;
-  const size_t smem = (size_t)SYMM_STAGES * SYMM_STAGE_BYTES;
-  SC_CUDA(cudaFuncSetAttribute(k_symm_dmma<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_symm_dmma<T><<<(unsigned)(row_blocks * splits), 256, smem, st>>>(s, rows, n, lds, t, ldt, b, row_blocks,
-                                                                cols_per_split, scratch, rows_pad);
+  if constexpr (std::is_same<T, __half>::value) {
+    const size_t smem = (size_t)SYMH_STAGES * SYMH_STAGE_BYTES;
+    SC_CUDA(cudaFuncSetAttribute(k_symm_dmma_f16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_symm_dmma_f16<<<(unsigned)(row_blocks * splits), 256, smem, st>>>(s, rows, n, lds, t, ldt, b, row_blocks,
+                                                                    cols_per_split, scratch, rows_pad);
+  } else {
+    const size_t smem = (size_t)SYMM_STAGES * SYMM_STAGE_BYTES;
+    SC_CUDA(cudaFuncSetAttribute(k_symm_dmma<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_symm_dmma<T><<<(unsigned)(row_blocks * splits), 256, smem, st>>>(s, rows, n, lds, t, ldt, b, row_blocks,
+                                                                  cols_per_split, scratch, rows_pad);
+  }
   sc::launched();
   k_symm_reduce<<<dim3((unsigned)((rows + 255) / 256), (unsigned)b), 256, 0, st>>>(scratch, splits, b, rows,
                                                                                  rows_pad, y, ldy);

@@ -39,13 +39,16 @@ FACTORED_PANEL_BYTES = 1 << 30
 # of the threshold pass and the 32-row bands of the blur); the blur reads 4 rows on either side.
 PANEL_ALIGN, BLUR_HALO = 128, 4
 # Bounded Diffuse (sc_diffuse_tile_list): the column groups of its row bounds, its output tile, and
-# the row order -- cosine k-means with this many clusters and passes on the rows' group-norm
-# profiles (the order only decides which tiles are skipped, never a value).
+# the row order -- spherical k-means on the device (sc_bound_order) with this many clusters and
+# assignment passes on the rows' group-norm profiles (the order only decides which tiles are
+# skipped, never a value; on the bench's speaker turns at N = 65,536 the tile count is the same
+# from 3 to 20 passes).
 BOUND_GROUP_COLS, LIST_BM, LIST_BN = 256, 128, 192
-BOUND_ORDER_CLUSTERS, BOUND_ORDER_ITERS = 16, 20
+BOUND_ORDER_CLUSTERS, BOUND_ORDER_ITERS = 16, 4
 # predict() takes the bounded Diffuse from this N (tools/time_bounded_diffuse.py, H100 80GB HBM3,
-# 700 W): at 16,384 its fixed costs (mostly the row order, 5.5 ms) leave it 25 % slower than the
-# storing Diffuse + stored solve (11.7 against 9.4 ms); at 32,768 it is 40 % faster (33 against 56).
+# 700 W, measured with the earlier host k-means row order): at 16,384 its fixed costs (mostly that
+# order, 5.5 ms) left it 25 % slower than the storing Diffuse + stored solve (11.7 against 9.4 ms);
+# at 32,768 it is 40 % faster (33 against 56).
 BOUNDED_FROM = 32768
 
 
@@ -440,16 +443,15 @@ class Engine:
     return norms, diag, c
 
   def bound_order(self, norms):
-    """Row order of the bounded Diffuse: stable sort of the cosine k-means labels of the profiles
-    (device int32).  Profiles k-means cannot seed (all rows alike) keep the natural order."""
+    """Row order of the bounded Diffuse (device int32): stable sort by the labels of a spherical
+    k-means of the profiles, computed and applied on the device without a host synchronisation.
+    The same order on every call; profiles that are all alike keep the natural order."""
     t = torch()
     n = int(norms.shape[0])
-    try:
-      labels, _ = self.kmeans(norms.double(), BOUND_ORDER_CLUSTERS, 0, BOUND_ORDER_ITERS)
-      perm = np.argsort(labels, kind="stable").astype(np.int32)
-    except ValueError:
-      perm = np.arange(n, dtype=np.int32)
-    return t.from_numpy(perm).to(self.device)
+    perm = t.empty(n, dtype=t.int32, device=self.device)
+    self.call("sc_bound_order", _ptr(norms), n, int(norms.shape[1]), BOUND_ORDER_CLUSTERS,
+              BOUND_ORDER_ITERS, _ptr(perm), self.stream)
+    return perm
 
   def rowmax_tiles(self, hi, n, norms, diag, perm):
     """Row maxima (fp32) of S = hi hi^T from the tiles of the product of hi[perm] that can hold
