@@ -195,6 +195,28 @@ int sc_diffuse_rowmax_tiles(sc_context* ctx, const void* yp_hi, int64_t ldh, int
  * Profiles that are all alike give the natural order. */
 int sc_bound_order(sc_context* ctx, const float* norms, int64_t n, int64_t groups, int k, int passes,
                    int* perm, void* stream);
+/* Hub-first bounded Diffuse (DESIGN.md section 3).
+ * sc_bound_order_hubs: the clusters of sc_bound_order, each re-sorted by its diagonal (diag, fp64,
+ * compared as fp32 rounded down) descending, ties by row; perm receives the rows in that order and
+ * starts (device int32 [k + 1]) the first position of each cluster, starts[k] = n.  The first row
+ * of a non-empty cluster is its hub.  Deterministic, enqueued only.  n <= 2^21.
+ * sc_diffuse_hub_tiles: phase 1, the tiles of each non-empty cluster's hub row block against the
+ * column blocks holding its rows, in the rasterised order and format of sc_diffuse_tile_list.
+ * sc_diffuse_tile_list_rows: phase 2, given rowmax = the maxima phase 1 folded (indexed by the
+ * original row): the tiles that straddle the diagonal or that the per-row rule keeps, minus the
+ * phase-1 tiles; *total receives the number of tiles of the full launch.
+ * sc_diffuse_rowmax_tiles_fold: sc_diffuse_rowmax_tiles folding into rowmax as it stands instead
+ * of zeroing it first. */
+int sc_bound_order_hubs(sc_context* ctx, const float* norms, int64_t n, int64_t groups, int k,
+                        int passes, const double* diag, int* perm, int* starts, void* stream);
+int sc_diffuse_hub_tiles(sc_context* ctx, const int* starts, int k, int64_t n, uint32_t* tiles,
+                         int* count, void* stream);
+int sc_diffuse_tile_list_rows(sc_context* ctx, const float* norms, int64_t groups, const int* perm,
+                              int64_t n, const float* rowmax, const int* starts, int k,
+                              uint32_t* tiles, int* count, int* total, void* stream);
+int sc_diffuse_rowmax_tiles_fold(sc_context* ctx, const void* yp_hi, int64_t ldh, int64_t n,
+                                 const uint32_t* tiles, const int* count, const int* perm,
+                                 float* rowmax, void* stream);
 
 /* Row maxima and row sums (fp64) of an fp32 matrix: the reductions of
  * RowWiseNormalize (refinement.py:243) and of the degree (laplacian.py:41). */

@@ -59,6 +59,11 @@ PROTOTYPES = {
     "sc_diffuse_tile_list": [c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_diffuse_rowmax_tiles": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_bound_order": [c_ptr, c_ptr, c_i64, c_i64, c_int, c_int, c_ptr, c_ptr],
+    "sc_bound_order_hubs": [c_ptr, c_ptr, c_i64, c_i64, c_int, c_int, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_diffuse_hub_tiles": [c_ptr, c_ptr, c_int, c_i64, c_ptr, c_ptr, c_ptr],
+    "sc_diffuse_tile_list_rows": [c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_ptr, c_ptr, c_int, c_ptr,
+                                  c_ptr, c_ptr, c_ptr],
+    "sc_diffuse_rowmax_tiles_fold": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_row_stats": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     "sc_affinity_stats": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr],
     "sc_row_normalize": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr],

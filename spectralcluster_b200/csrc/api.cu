@@ -35,7 +35,12 @@ int diffuse_tile_list(const float* norms, int G, const double* diag_lb, const in
                       int64_t n, uint32_t* list, int* count, int* total, cudaStream_t st);
 int diffuse_rowmax_tiles(const sc_context* ctx, const __half* y_hi, int64_t ldh, int64_t n,
                          const uint32_t* list, const int* count, const int* row_map,
-                         float* rowmax, cudaStream_t st);
+                         float* rowmax, bool fold, cudaStream_t st);
+int diffuse_hub_tiles(const int* starts, int k, int64_t n, uint32_t* list, int* count,
+                      cudaStream_t st);
+int diffuse_tile_list_rows(const float* norms, int G, const int* perm, int64_t n,
+                           const float* rowmax, const int* starts, int k, uint32_t* list,
+                           int* count, int* total, cudaStream_t st);
 // rowops.cu
 int crop_diagonal_rows(const float* a, int64_t n, int64_t lda, int64_t row_begin, int64_t rows,
                        float* diag_out, cudaStream_t st);
@@ -160,7 +165,32 @@ extern "C" int sc_diffuse_rowmax_tiles(sc_context* ctx, const void* yp_hi, int64
   SC_REQUIRE(ctx && yp_hi && tiles && count && perm && rowmax && n > 0,
              "sc_diffuse_rowmax_tiles: bad arguments");
   return diffuse_rowmax_tiles(ctx, (const __half*)yp_hi, ldh, n, tiles, count, perm, rowmax,
-                              as_stream(stream));
+                              false, as_stream(stream));
+}
+
+extern "C" int sc_diffuse_rowmax_tiles_fold(sc_context* ctx, const void* yp_hi, int64_t ldh,
+                                            int64_t n, const uint32_t* tiles, const int* count,
+                                            const int* perm, float* rowmax, void* stream) {
+  SC_REQUIRE(ctx && yp_hi && tiles && count && perm && rowmax && n > 0,
+             "sc_diffuse_rowmax_tiles_fold: bad arguments");
+  return diffuse_rowmax_tiles(ctx, (const __half*)yp_hi, ldh, n, tiles, count, perm, rowmax,
+                              true, as_stream(stream));
+}
+
+extern "C" int sc_diffuse_hub_tiles(sc_context* ctx, const int* starts, int k, int64_t n,
+                                    uint32_t* tiles, int* count, void* stream) {
+  SC_REQUIRE(ctx && starts && tiles && count && n > 0, "sc_diffuse_hub_tiles: bad arguments");
+  return diffuse_hub_tiles(starts, k, n, tiles, count, as_stream(stream));
+}
+
+extern "C" int sc_diffuse_tile_list_rows(sc_context* ctx, const float* norms, int64_t groups,
+                                         const int* perm, int64_t n, const float* rowmax,
+                                         const int* starts, int k, uint32_t* tiles, int* count,
+                                         int* total, void* stream) {
+  SC_REQUIRE(ctx && norms && perm && rowmax && starts && tiles && count && total && n > 0,
+             "sc_diffuse_tile_list_rows: bad arguments");
+  return diffuse_tile_list_rows(norms, (int)groups, perm, n, rowmax, starts, k, tiles, count,
+                                total, as_stream(stream));
 }
 
 // ---- row-block / general variants used by the row-sharded multi-GPU pipeline ----------------

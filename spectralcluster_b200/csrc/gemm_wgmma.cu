@@ -871,9 +871,168 @@ int diffuse_tile_list(const float* norms, int G, const double* diag_lb, const in
   return 0;
 }
 
+// ---- hub-first bounded Diffuse (DESIGN.md section 3).  The rows are ordered cluster by cluster,
+// each cluster's row of largest diagonal (its hub) first; starts[c] is the first row of cluster c in
+// that order, starts[k] = n.  Phase 1 computes, for every non-empty cluster [s, e), the tiles of the
+// hub's row block against the column blocks that hold its rows: every row of the cluster then has
+// its element with the hub folded into its maximum L_i.  Phase 2 keeps a tile iff it straddles the
+// diagonal or some row i of it has (1 + eps) u_iJ >= L_i, u_iJ = sum_g |y_i^g| max_{j in J} |y_j^g|
+// (or some column j the same with the roles swapped), and phase 1 did not compute it.
+__device__ __forceinline__ bool is_hub_tile(int m, int c, const int* __restrict__ starts, int k) {
+  for (int q = 0; q < k; ++q) {
+    const int s = starts[q], e = starts[q + 1];
+    if (e > s && s / BM == m && s / LIST_BN <= c && c <= (e - 1) / LIST_BN) return true;
+  }
+  return false;
+}
+
+// flags[m tiles_n + c]: phase 1 (rule_row == nullptr) = the hub tiles; phase 2 = the straddling
+// tiles and those the row rule keeps, minus the hub tiles.  Tiles below the diagonal are never read.
+__global__ void k_hub_tile_flags(const int* __restrict__ starts, int k, int tiles_m, int tiles_n,
+                                 const uint8_t* __restrict__ rule_row,
+                                 const uint8_t* __restrict__ rule_col, uint8_t* __restrict__ flags) {
+  const int64_t id = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (id >= (int64_t)tiles_m * tiles_n) return;
+  const int m = (int)(id / tiles_n), c = (int)(id - (int64_t)m * tiles_n);
+  const bool hub = is_hub_tile(m, c, starts, k);
+  bool keep;
+  if (rule_row == nullptr)
+    keep = hub;
+  else if (hub || (int64_t)c * LIST_BN + LIST_BN - 1 < (int64_t)m * BM)
+    keep = false;
+  else
+    keep = (int64_t)c * LIST_BN < (int64_t)m * BM + BM || rule_row[id] ||
+           rule_col[(int64_t)c * tiles_m + m];
+  flags[id] = keep ? 1 : 0;
+}
+
+// The per-row rule as one dense product over the permuted rows: CTA (b, t0) takes the R rows of
+// block b and the other side's blocks t0 .. t0 + 31, whose group-norm maxima are omax [T, G].
+// out[b T + t] = 1 iff some row i of block b has (1 + eps) sum_g |y_i^g| omax[t][g] >= L_i (fp64,
+// every operation rounded up; L_i = rowmax[perm[i]] exactly).  row_side: block b is a row block
+// (R = 128) against column blocks (192); otherwise a column block against row blocks.  Only the
+// pairs that form a tile wholly above the diagonal are wanted; CTAs without one return at once.
+constexpr int RULE_T = 32, RULE_GC = 32;
+
+template <int R>
+__global__ void __launch_bounds__(256) k_row_rule(const float* __restrict__ norms, int G,
+                                                  const int* __restrict__ perm, int n,
+                                                  const float* __restrict__ rowmax,
+                                                  const float* __restrict__ omax, int T,
+                                                  bool row_side, uint8_t* __restrict__ out) {
+  constexpr int RO = (R == BM) ? LIST_BN : BM;      // rows per block of the other side
+  constexpr int RQ = R / 16;                        // rows per thread
+  __shared__ float sn[R][RULE_GC + 1];
+  __shared__ float so[RULE_GC][RULE_T];
+  __shared__ int fl[RULE_T];
+  const int b = blockIdx.x, t0 = blockIdx.y * RULE_T;
+  // wanted pair (b, t): row side  RO t >= R b + R;  column side  R b >= RO t + RO
+  const bool any = row_side ? (int64_t)RO * min(T - 1, t0 + RULE_T - 1) >= (int64_t)R * b + R
+                            : (int64_t)R * b >= (int64_t)RO * t0 + RO;
+  if (!any) return;
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  if (threadIdx.x < RULE_T) fl[threadIdx.x] = 0;
+  double acc[RQ][2];
+#pragma unroll
+  for (int q = 0; q < RQ; ++q) acc[q][0] = acc[q][1] = 0.0;
+  for (int g0 = 0; g0 < G; g0 += RULE_GC) {
+    __syncthreads();
+    for (int e = threadIdx.x; e < R * RULE_GC; e += blockDim.x) {
+      const int r = e / RULE_GC, g = g0 + e % RULE_GC;
+      const int i = b * R + r;
+      sn[r][e % RULE_GC] = (i < n && g < G) ? norms[(int64_t)perm[i] * G + g] : 0.f;
+    }
+    for (int e = threadIdx.x; e < RULE_T * RULE_GC; e += blockDim.x) {
+      const int t = e / RULE_GC, g = g0 + e % RULE_GC;
+      so[e % RULE_GC][t] = (t0 + t < T && g < G) ? omax[(int64_t)(t0 + t) * G + g] : 0.f;
+    }
+    __syncthreads();
+#pragma unroll 4
+    for (int g = 0; g < RULE_GC; ++g) {
+      const double o0 = (double)so[g][tx], o1 = (double)so[g][tx + 16];
+#pragma unroll
+      for (int q = 0; q < RQ; ++q) {
+        const double v = (double)sn[ty + 16 * q][g];
+        acc[q][0] = __fma_ru(v, o0, acc[q][0]);
+        acc[q][1] = __fma_ru(v, o1, acc[q][1]);
+      }
+    }
+  }
+  bool k0 = false, k1 = false;
+#pragma unroll
+  for (int q = 0; q < RQ; ++q) {
+    const int i = b * R + ty + 16 * q;
+    if (i < n) {
+      const double l = (double)rowmax[perm[i]];
+      k0 |= !(__dmul_ru(acc[q][0], 1.0 + BOUND_EPS) < l);
+      k1 |= !(__dmul_ru(acc[q][1], 1.0 + BOUND_EPS) < l);
+    }
+  }
+  if (k0) fl[tx] = 1;
+  if (k1) fl[tx + 16] = 1;
+  __syncthreads();
+  if (threadIdx.x < RULE_T && t0 + (int)threadIdx.x < T)
+    out[(int64_t)b * T + t0 + threadIdx.x] = (uint8_t)fl[threadIdx.x];
+}
+
+int diffuse_hub_tiles(const int* starts, int k, int64_t n, uint32_t* list, int* count,
+                      cudaStream_t st) {
+  SC_REQUIRE(n > 0 && n <= BOUND_MAX_K && k >= 1 && k <= 16,
+             "sc_diffuse_hub_tiles: n must lie in [1, 2^20] and k in [1, 16]");
+  const int tiles_m = (int)((n + BM - 1) / BM), tiles_n = (int)((n + LIST_BN - 1) / LIST_BN);
+  const int64_t tiles = (int64_t)tiles_m * tiles_n;
+  Scratch flags, total;
+  SC_CUDA(flags.alloc((size_t)tiles, st));
+  SC_CUDA(total.alloc(sizeof(int), st));
+  k_hub_tile_flags<<<(unsigned)((tiles + 255) / 256), 256, 0, st>>>(starts, k, tiles_m, tiles_n,
+                                                                   nullptr, nullptr,
+                                                                   flags.as<uint8_t>());
+  k_tile_compact<<<1, 1024, 0, st>>>(flags.as<uint8_t>(), tiles_m, tiles_n, list, count,
+                                     total.as<int>());
+  sc::launched(2);
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
+int diffuse_tile_list_rows(const float* norms, int G, const int* perm, int64_t n,
+                           const float* rowmax, const int* starts, int k, uint32_t* list,
+                           int* count, int* total, cudaStream_t st) {
+  SC_REQUIRE(n > 0 && n <= BOUND_MAX_K && G == (n + 255) / 256 && k >= 1 && k <= 16,
+             "sc_diffuse_tile_list_rows: n must lie in [1, 2^20], G = ceil(n / 256), k in [1, 16]");
+  const int tiles_m = (int)((n + BM - 1) / BM), tiles_n = (int)((n + LIST_BN - 1) / LIST_BN);
+  const int64_t tiles = (int64_t)tiles_m * tiles_n;
+  Scratch amax, bmax, amin, bmin, diag0, rule_row, rule_col, flags;
+  SC_CUDA(amax.alloc(sizeof(float) * tiles_m * G, st));
+  SC_CUDA(bmax.alloc(sizeof(float) * tiles_n * G, st));
+  SC_CUDA(amin.alloc(sizeof(double) * tiles_m, st));
+  SC_CUDA(bmin.alloc(sizeof(double) * tiles_n, st));
+  SC_CUDA(diag0.alloc(sizeof(double) * n, st));
+  SC_CUDA(rule_row.alloc((size_t)tiles, st));
+  SC_CUDA(rule_col.alloc((size_t)tiles, st));
+  SC_CUDA(flags.alloc((size_t)tiles, st));
+  // the block maxima of the norms (the block minima of k_block_bounds are not used here: a zeroed
+  // diagonal stands in for them)
+  SC_CUDA(cudaMemsetAsync(diag0.p, 0, sizeof(double) * n, st));
+  k_block_bounds<<<tiles_m, 256, 0, st>>>(norms, G, diag0.as<double>(), perm, (int)n, BM,
+                                          amax.as<float>(), amin.as<double>());
+  k_block_bounds<<<tiles_n, 256, 0, st>>>(norms, G, diag0.as<double>(), perm, (int)n, LIST_BN,
+                                          bmax.as<float>(), bmin.as<double>());
+  k_row_rule<BM><<<dim3(tiles_m, (tiles_n + RULE_T - 1) / RULE_T), 256, 0, st>>>(
+      norms, G, perm, (int)n, rowmax, bmax.as<float>(), tiles_n, true, rule_row.as<uint8_t>());
+  k_row_rule<LIST_BN><<<dim3(tiles_n, (tiles_m + RULE_T - 1) / RULE_T), 256, 0, st>>>(
+      norms, G, perm, (int)n, rowmax, amax.as<float>(), tiles_m, false, rule_col.as<uint8_t>());
+  k_hub_tile_flags<<<(unsigned)((tiles + 255) / 256), 256, 0, st>>>(
+      starts, k, tiles_m, tiles_n, rule_row.as<uint8_t>(), rule_col.as<uint8_t>(),
+      flags.as<uint8_t>());
+  k_tile_compact<<<1, 1024, 0, st>>>(flags.as<uint8_t>(), tiles_m, tiles_n, list, count, total);
+  sc::launched(6);
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
 int diffuse_rowmax_tiles(const sc_context* ctx, const __half* y_hi, int64_t ldh, int64_t n,
                          const uint32_t* list, const int* count, const int* row_map,
-                         float* rowmax, cudaStream_t st) {
+                         float* rowmax, bool fold, cudaStream_t st) {
   SC_REQUIRE(n > 0 && n <= BOUND_MAX_K, "sc_diffuse_rowmax_tiles: n must lie in [1, 2^20]");
   constexpr int PREC = 1, BN = LIST_BN;
   constexpr int STAGES = StageGeom<PREC, BN>::STAGES;
@@ -885,7 +1044,7 @@ int diffuse_rowmax_tiles(const sc_context* ctx, const __half* y_hi, int64_t ldh,
   SC_REQUIRE(smem <= ctx->smem_optin, "wgmma GEMM needs %zu B of shared memory", smem);
   auto kern = k_gemm_wgmma<PREC, TC_EPI_PLAIN, true, BN, true>;
   SC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  SC_CUDA(cudaMemsetAsync(rowmax, 0, sizeof(float) * n, st));
+  if (!fold) SC_CUDA(cudaMemsetAsync(rowmax, 0, sizeof(float) * n, st));
   int grid = ctx->sm_count;
   if (ctx->gemm_sm_limit > 0 && ctx->gemm_sm_limit < grid) grid = ctx->gemm_sm_limit;
   // the tile count is on the device: pace whenever K is long enough (CTAs without a tile sign off

@@ -298,27 +298,91 @@ __global__ void k_order_scan(const int* __restrict__ counts, int chunks, int k, 
   for (int p = 0; p < chunks; ++p) base[(size_t)p * k + j] += off;
 }
 
-}  // namespace sc
+// ---- hub-first order (sc_bound_order_hubs): within each cluster, rows by diagonal descending.
+// Key = label (bits 52..55) | complement of the fp32 diagonal rounded down (bits 21..51) | row
+// (bits 0..20): ascending keys are (label, diagonal descending, row), distinct for every row.
+constexpr int HUB_SORT_LOCAL = 2048;   // keys a CTA sorts or merges in shared memory (1024 threads)
 
-using namespace sc;
+__global__ void k_hub_keys(const int* __restrict__ labels, const double* __restrict__ diag,
+                           int64_t n, int64_t P, unsigned long long* __restrict__ keys) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P) return;
+  if (i >= n) { keys[i] = ~0ull; return; }
+  const unsigned d = __float_as_uint(__double2float_rd(diag[i])) & 0x7fffffffu;
+  keys[i] = ((unsigned long long)labels[i] << 52) |
+            ((unsigned long long)(0x7fffffffu - d) << 21) | (unsigned long long)i;
+}
 
-extern "C" int sc_bound_order(sc_context* ctx, const float* norms, int64_t n, int64_t groups, int k,
-                              int passes, int* perm, void* stream) {
-  SC_REQUIRE(ctx && norms && perm && n > 0 && n <= (1LL << 30) && groups > 0 && k >= 1 &&
-             k <= ORDER_MAXK && passes >= 1, "sc_bound_order: bad arguments");
+__device__ __forceinline__ void hub_cas(unsigned long long* s, int i, int j, bool asc) {
+  const unsigned long long a = s[i], b = s[j];
+  if ((a > b) == asc) { s[i] = b; s[j] = a; }
+}
+
+// bitonic steps with partner distance < L = min(P, HUB_SORT_LOCAL) in shared memory: stages
+// 2..L from scratch (merge_k == 0), or the tail j = L/2 .. 1 of stage merge_k
+__global__ void __launch_bounds__(1024) k_hub_sort_local(unsigned long long* __restrict__ keys,
+                                                         int64_t P, int64_t merge_k) {
+  __shared__ unsigned long long s[HUB_SORT_LOCAL];
+  const int L = (int)min(P, (int64_t)HUB_SORT_LOCAL);
+  const int64_t base = (int64_t)blockIdx.x * L;
+  for (int i = threadIdx.x; i < L; i += blockDim.x) s[i] = keys[base + i];
+  __syncthreads();
+  for (int64_t k = merge_k ? merge_k : 2; k <= (merge_k ? merge_k : (int64_t)L); k <<= 1) {
+    for (int j = (int)min(k >> 1, (int64_t)L >> 1); j > 0; j >>= 1) {
+      for (int i = threadIdx.x; i < L; i += blockDim.x) {
+        const int p = i ^ j;
+        if (p > i) hub_cas(s, i, p, ((base + i) & k) == 0);
+      }
+      __syncthreads();
+    }
+  }
+  for (int i = threadIdx.x; i < L; i += blockDim.x) keys[base + i] = s[i];
+}
+
+// one bitonic step of stage k at partner distance j >= HUB_SORT_LOCAL, in global memory
+__global__ void k_hub_sort_step(unsigned long long* __restrict__ keys, int64_t P, int64_t k,
+                                int64_t j) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= P) return;
+  const int64_t p = i ^ j;
+  if (p > i) {
+    const unsigned long long a = keys[i], b = keys[p];
+    if ((a > b) == ((i & k) == 0)) { keys[i] = b; keys[p] = a; }
+  }
+}
+
+// perm = the rows of the sorted keys; starts[j] = base[0][j] (rows of labels < j), starts[k] = n
+__global__ void k_hub_finish(const unsigned long long* __restrict__ keys, int64_t n,
+                             const int* __restrict__ base, int k, int* __restrict__ perm,
+                             int* __restrict__ starts) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) perm[i] = (int)(keys[i] & 0x1fffffull);
+  if (i <= k) starts[i] = i < k ? base[i] : (int)n;
+}
+
+// The k-means of both orders: labels[i] of every row, with the seeding and passes described at
+// the top of this file.  `buf` receives the scratch; labels, counts and base point into it.
+struct OrderScratch {
+  Scratch buf;
+  int* labels;
+  int* counts;
+  int* base;
+  int chunks;
+};
+
+static int order_labels(sc_context* ctx, const char* who, const float* norms, int64_t n,
+                        int64_t groups, int k, int passes, size_t extra, OrderScratch& o,
+                        cudaStream_t st) {
   const size_t smem = sizeof(float) * 2 * (size_t)k * (size_t)groups;
   SC_REQUIRE(smem <= ctx->smem_optin - 2 * sizeof(int) * ORDER_CHUNK,
-             "sc_bound_order: %d centres of %lld groups do not fit in shared memory", k,
-             (long long)groups);
-  cudaStream_t st = as_stream(stream);
+             "%s: %d centres of %lld groups do not fit in shared memory", who, k, (long long)groups);
   const int G = (int)groups;
   const int chunks = (int)((n + ORDER_CHUNK - 1) / ORDER_CHUNK);
   const size_t cbytes = sizeof(float) * (size_t)k * G;
   const size_t pbytes = cbytes * (size_t)chunks;
-  Scratch buf;
-  SC_CUDA(buf.alloc(cbytes + pbytes + sizeof(float) * 2 * (size_t)n + sizeof(int) * (size_t)n +
-                        sizeof(float2) * chunks + sizeof(int) * 2 * (size_t)chunks * k + 64, st));
-  char* p = buf.as<char>();
+  SC_CUDA(o.buf.alloc(extra + cbytes + pbytes + sizeof(float) * 2 * (size_t)n + sizeof(int) * (size_t)n +
+                          sizeof(float2) * chunks + sizeof(int) * 2 * (size_t)chunks * k + 64, st));
+  char* p = o.buf.as<char>() + extra;
   float* c = reinterpret_cast<float*>(p);                     p += cbytes;
   float* part = reinterpret_cast<float*>(p);                  p += pbytes;
   float* rn = reinterpret_cast<float*>(p);                    p += sizeof(float) * n;
@@ -328,6 +392,10 @@ extern "C" int sc_bound_order(sc_context* ctx, const float* norms, int64_t n, in
   float2* cand = reinterpret_cast<float2*>(p);                p += sizeof(float2) * chunks;
   int* counts = reinterpret_cast<int*>(p);                    p += sizeof(int) * (size_t)chunks * k;
   int* base = reinterpret_cast<int*>(p);
+  o.labels = labels;
+  o.counts = counts;
+  o.base = base;
+  o.chunks = chunks;
 
   k_order_seed0<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(norms, n, G, rn, c); sc::launched();
   for (int j = 1; j < k; ++j) {
@@ -346,9 +414,52 @@ extern "C" int sc_bound_order(sc_context* ctx, const float* norms, int64_t n, in
       k_order_update<<<(unsigned)k, 256, sizeof(float) * G, st>>>(part, chunks, G, k, c); sc::launched();
     }
   }
+  // per-chunk label counts and their exclusive scan in (label, chunk) order
   k_order_rank<<<(unsigned)chunks, ORDER_CHUNK, 0, st>>>(labels, n, k, counts, nullptr, nullptr); sc::launched();
   k_order_scan<<<1, ORDER_MAXK, 0, st>>>(counts, chunks, k, base); sc::launched();
-  k_order_rank<<<(unsigned)chunks, ORDER_CHUNK, 0, st>>>(labels, n, k, nullptr, base, perm); sc::launched();
+  return 0;
+}
+
+}  // namespace sc
+
+using namespace sc;
+
+extern "C" int sc_bound_order(sc_context* ctx, const float* norms, int64_t n, int64_t groups, int k,
+                              int passes, int* perm, void* stream) {
+  SC_REQUIRE(ctx && norms && perm && n > 0 && n <= (1LL << 30) && groups > 0 && k >= 1 &&
+             k <= ORDER_MAXK && passes >= 1, "sc_bound_order: bad arguments");
+  cudaStream_t st = as_stream(stream);
+  OrderScratch o;
+  if (int r = order_labels(ctx, "sc_bound_order", norms, n, groups, k, passes, 0, o, st)) return r;
+  k_order_rank<<<(unsigned)o.chunks, ORDER_CHUNK, 0, st>>>(o.labels, n, k, nullptr, o.base, perm); sc::launched();
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int sc_bound_order_hubs(sc_context* ctx, const float* norms, int64_t n, int64_t groups,
+                                   int k, int passes, const double* diag, int* perm, int* starts,
+                                   void* stream) {
+  SC_REQUIRE(ctx && norms && diag && perm && starts && n > 0 && n <= (1LL << 21) && groups > 0 &&
+             k >= 1 && k <= ORDER_MAXK && passes >= 1, "sc_bound_order_hubs: bad arguments");
+  cudaStream_t st = as_stream(stream);
+  int64_t P = 2;
+  while (P < n) P <<= 1;
+  const size_t kbytes = sizeof(unsigned long long) * (size_t)P;
+  OrderScratch o;
+  if (int r = order_labels(ctx, "sc_bound_order_hubs", norms, n, groups, k, passes, kbytes, o, st))
+    return r;
+  unsigned long long* keys = o.buf.as<unsigned long long>();
+  k_hub_keys<<<(unsigned)((P + 255) / 256), 256, 0, st>>>(o.labels, diag, n, P, keys); sc::launched();
+  const int64_t L = P < HUB_SORT_LOCAL ? P : HUB_SORT_LOCAL;
+  const unsigned blocks = (unsigned)(P / L);
+  k_hub_sort_local<<<blocks, 1024, 0, st>>>(keys, P, 0); sc::launched();
+  for (int64_t kk = 2 * L; kk <= P; kk <<= 1) {
+    for (int64_t j = kk >> 1; j >= L; j >>= 1) {
+      k_hub_sort_step<<<(unsigned)((P + 255) / 256), 256, 0, st>>>(keys, P, kk, j); sc::launched();
+    }
+    k_hub_sort_local<<<blocks, 1024, 0, st>>>(keys, P, kk); sc::launched();
+  }
+  k_hub_finish<<<(unsigned)((n + 256) / 256), 256, 0, st>>>(keys, n, o.base, k, perm, starts); sc::launched();
   SC_LAUNCH_CHECK();
   return 0;
 }

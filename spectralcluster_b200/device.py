@@ -470,20 +470,62 @@ class Engine:
     del yp
     return mx, counts
 
+  def bound_order_hubs(self, norms, diag):
+    """Hub-first row order of the bounded Diffuse: the clusters of bound_order, each re-sorted by
+    its diagonal descending (ties by row), as (perm, starts) device int32 tensors; starts[c] is the
+    first position of cluster c and starts[-1] = n.  No host synchronisation."""
+    t = torch()
+    n = int(norms.shape[0])
+    perm = t.empty(n, dtype=t.int32, device=self.device)
+    starts = t.empty(BOUND_ORDER_CLUSTERS + 1, dtype=t.int32, device=self.device)
+    self.call("sc_bound_order_hubs", _ptr(norms), n, int(norms.shape[1]), BOUND_ORDER_CLUSTERS,
+              BOUND_ORDER_ITERS, _ptr(diag), _ptr(perm), _ptr(starts), self.stream)
+    return perm, starts
+
+  def hub_rowmax_tiles(self, hi, n, norms, perm, starts, want_phase1=False):
+    """Row maxima (fp32) of S = hi hi^T in two listed launches over hi[perm]: phase 1 pairs every
+    cluster's rows with its hub, phase 2 computes the tiles the per-row rule keeps against the
+    maxima phase 1 found.  Also the tile counts (phase 1, phase 2, total) as a device int32 [3],
+    and with want_phase1 a copy of the phase-1 maxima."""
+    t = torch()
+    yp = t.empty_like(hi)
+    self.call("sc_gather_rows_f16", _ptr(hi), hi.stride(0), _ptr(perm), n, hi.shape[1], _ptr(yp),
+              yp.stride(0), self.stream)
+    k = int(starts.shape[0]) - 1
+    size = -(-n // LIST_BM) * -(-n // LIST_BN)
+    tiles1 = t.empty(size, dtype=t.int32, device=self.device)
+    tiles2 = t.empty(size, dtype=t.int32, device=self.device)
+    counts = t.empty(3, dtype=t.int32, device=self.device)
+    mx = self.vector(n, t.float32)
+    self.call("sc_diffuse_hub_tiles", _ptr(starts), k, n, _ptr(tiles1), _ptr(counts), self.stream)
+    self.call("sc_diffuse_rowmax_tiles", _ptr(yp), yp.stride(0), n, _ptr(tiles1), _ptr(counts),
+              _ptr(perm), _ptr(mx), self.stream)
+    phase1 = mx.clone() if want_phase1 else None
+    self.call("sc_diffuse_tile_list_rows", _ptr(norms), int(norms.shape[1]), _ptr(perm), n,
+              _ptr(mx), _ptr(starts), k, _ptr(tiles2), _ptr(counts[1:]), _ptr(counts[2:]),
+              self.stream)
+    self.call("sc_diffuse_rowmax_tiles_fold", _ptr(yp), yp.stride(0), n, _ptr(tiles2),
+              _ptr(counts[1:]), _ptr(perm), _ptr(mx), self.stream)
+    del yp
+    if want_phase1:
+      return mx, counts, phase1
+    return mx, counts
+
   def bounded_diffuse(self, n, hi, want_max=True):
     """Statistics of S = Y Y^T (Y >= 0 and bitwise symmetric, `hi` its fp16 plane), S never formed:
     (rowmax fp32 or None, rowsum fp64, tile counts).  rowsum = Y (Y 1) by two passes over Y; the
-    row maxima, when wanted, from the bounded tile list (bit for bit those of sc_diffuse).  The
-    counts are an int32 tensor [2] (computed, total): on the device, or on the host (0 computed)
-    when no GEMM runs."""
+    row maxima, when wanted, from the hub-first tile lists (bit for bit those of sc_diffuse).  The
+    counts are an int32 tensor [2] (computed in both phases, total): on the device, or on the host
+    (0 computed) when no GEMM runs."""
     t = torch()
     norms, diag, c = self.row_group_bounds(hi, n)
     rowsum = t.empty((1, n), dtype=t.float64, device=self.device)
     self.block_product_f16(hi, n, n, c.view(1, -1), 1, rowsum)
     if not want_max:
       return None, rowsum.view(n), t.tensor([0, bounded_tile_count(n)], dtype=t.int32)
-    mx, counts = self.rowmax_tiles(hi, n, norms, diag, self.bound_order(norms))
-    return mx, rowsum.view(n), counts
+    perm, starts = self.bound_order_hubs(norms, diag)
+    mx, counts = self.hub_rowmax_tiles(hi, n, norms, perm, starts)
+    return mx, rowsum.view(n), t.stack((counts[0] + counts[1], counts[2]))
 
   # ---- row panels of the factored route
   def normalized_planes(self, x_dev):

@@ -5,7 +5,8 @@
 For each N: Y_hi of the ICASSP front end on the bench's speaker-turn generator (seed 0), then per
 repetition the old back end (storing sc_diffuse with its epilogue statistics + sc_eigh_extremal on
 S) and the new one (row bounds + row sums, row order, gather + tile list + listed GEMM, then
-sc_eigh_extremal_factored), each stage bracketed by CUDA events.  Reports per-stage ms, the share of
+sc_eigh_extremal_factored), and the hub-first route (hub order, phase-1 and phase-2 lists and
+GEMMs), each stage bracketed by CUDA events.  Reports per-stage ms, the share of
 tiles computed and the TFLOP/s of the computed tiles (128 x 192 x N multiply-adds each), and the
 same for an input where nothing can be skipped (identical rows), the worst-case overhead.
 """
@@ -74,8 +75,23 @@ def new_route(eng, n, hi):
   return st
 
 
+def hub_route(eng, n, hi):
+  st = {}
+  norms, diag, c = timed(st, "bounds", lambda: eng.row_group_bounds(hi, n))
+  rowsum = torch.empty((1, n), dtype=torch.float64, device=eng.device)
+  timed(st, "rowsum", lambda: eng.block_product_f16(hi, n, n, c.view(1, -1), 1, rowsum))
+  perm, starts = timed(st, "order", lambda: eng.bound_order_hubs(norms, diag))
+  mx, counts = timed(st, "tiles+gemm", lambda: eng.hub_rowmax_tiles(hi, n, norms, perm, starts))
+  r = dev.Refined(None, n, True, 1.0 / mx.double(), rowsum.view(n), y_hi=hi)
+  delta, left, right, sign, which = lap.operator_terms(eng, r, scb.LaplacianType.GraphCut)
+  timed(st, "eigensolve", lambda: eng.eigh_factored(hi, n, delta, left, right, sign, which, 11, 11))
+  p1, p2, total = counts.tolist()
+  st["tiles"], st["of"], st["phase1"] = p1 + p2, total, p1
+  return st
+
+
 def summarise(runs):
-  keys = [k for k in runs[0] if k not in ("tiles", "of")]
+  keys = [k for k in runs[0] if k not in ("tiles", "of", "phase1")]
   out = {k: float(np.median([r[k] for r in runs])) for k in keys}
   out["total"] = float(np.median([sum(r[k] for k in keys) for r in runs]))
   return out
@@ -97,18 +113,22 @@ def main():
       else:
         hi = torch.zeros((n, dev.round_up(n, 64)), dtype=torch.float16, device=eng.device)
         hi[:, :n] = 0.125
-      old_route(eng, n, hi), new_route(eng, n, hi)          # warm-up
-      olds, news = [], []
+      old_route(eng, n, hi), new_route(eng, n, hi), hub_route(eng, n, hi)   # warm-up
+      olds, news, hubs = [], [], []
       for _ in range(args.reps):
         olds.append(old_route(eng, n, hi))
         news.append(new_route(eng, n, hi))
-      new = summarise(news)
-      computed, total = news[-1]["tiles"], news[-1]["of"]
-      flop = 2.0 * dev.LIST_BM * dev.LIST_BN * n * computed
-      report["sizes"].setdefault(str(n), {})[kind] = {
-          "old_ms": summarise(olds), "new_ms": new,
-          "tiles": computed, "of": total, "tile_fraction": computed / total,
-          "computed_tile_TFLOPs": flop / (new["tiles+gemm"] * 1e-3) / 1e12}
+        hubs.append(hub_route(eng, n, hi))
+      entry = {"old_ms": summarise(olds)}
+      for name, runs in (("tile_wide", news), ("hub", hubs)):
+        ms = summarise(runs)
+        computed, total = runs[-1]["tiles"], runs[-1]["of"]
+        flop = 2.0 * dev.LIST_BM * dev.LIST_BN * n * computed
+        entry[name] = {"ms": ms, "tiles": computed, "of": total, "tile_fraction": computed / total,
+                       "computed_tile_TFLOPs": flop / (ms["tiles+gemm"] * 1e-3) / 1e12}
+        if name == "hub":
+          entry[name]["phase1_tiles"] = runs[-1]["phase1"]
+      report["sizes"].setdefault(str(n), {})[kind] = entry
       print(json.dumps({str(n): {kind: report["sizes"][str(n)][kind]}}), flush=True)
       del hi
       torch.cuda.empty_cache()
