@@ -229,6 +229,18 @@ int sc_row_stats(sc_context* ctx, const float* a, int64_t n, int64_t lda, double
 int sc_affinity_stats(sc_context* ctx, const float* a, int64_t n, int64_t lda, double* out_host,
                       void* stream);
 
+/* The same reductions over an affinity that is never stored (the factored route), built in row
+ * panels.  sc_affinity_stats_rows takes rows [row_begin, row_begin + rows) of the affinity as the
+ * fp32 panel [rows, ldp] and writes their per-row partials into the DEVICE fp64 buffer part
+ * [4 n + 4] (the row kernel of sc_affinity_stats, plus a[i][i+1] per row).  Once every row has
+ * been through it, sc_affinity_stats_finish reduces part in sc_affinity_stats's fixed order, so
+ * out_host[0..4) equals what sc_affinity_stats returns on the whole matrix, bit for bit.
+ * sc_affinity_stats_finish is SYNCHRONOUS. */
+int sc_affinity_stats_rows(sc_context* ctx, const float* panel, int64_t rows, int64_t n,
+                           int64_t ldp, int64_t row_begin, double* part, void* stream);
+int sc_affinity_stats_finish(sc_context* ctx, double* part, int64_t n, double* out_host,
+                             void* stream);
+
 /* RowWiseNormalize.refine (refinement.py:240-245), materialised.  out may alias a. */
 int sc_row_normalize(sc_context* ctx, const float* a, int64_t n, int64_t lda, float* out,
                      int64_t ldo, void* stream);
@@ -623,6 +635,23 @@ enum sc_gmm_mode {
 };
 int sc_gmm_band_pass(sc_context* ctx, const float* a, int64_t n, int64_t lda, int64_t offset,
                      int mode, const double* params_host, double* work, double* out_host,
+                     void* stream);
+
+/* The packed band, for an affinity that is never stored (the factored route).  Row i of the band,
+ * j0 = max(0, i + offset) < n, keeps columns [c0, n), c0 = j0 & ~3, at band[row_off[i] ...], with
+ * row_off[i] % 4 == 0 and row_off[i + 1] = row_off[i] + round_up(n - c0, 4) (0 for rows without
+ * band elements); row_off is a DEVICE int64 array [n + 1] (gmm_bic.packed_row_offsets).  Column j
+ * has the position mod 4 it has in a dense [n, lda] matrix, so sc_gmm_band_pass_packed reads the
+ * same samples in the same order as sc_gmm_band_pass and returns the same out_host, bit for bit;
+ * its modes, params, work and out are those of sc_gmm_band_pass.  SYNCHRONOUS.
+ * sc_gmm_band_pack copies rows [row_begin, row_begin + rows) of the matrix, given as the fp32 panel
+ * [rows, ldp] (ldp >= round_up(n, 4)), into their packed rows, with NaN in the slots [c0, j0) and
+ * [n, round_up(n, 4)). */
+int sc_gmm_band_pass_packed(sc_context* ctx, const float* band, const int64_t* row_off, int64_t n,
+                            int64_t offset, int mode, const double* params_host, double* work,
+                            double* out_host, void* stream);
+int sc_gmm_band_pack(sc_context* ctx, const float* panel, int64_t ldp, int64_t row_begin,
+                     int64_t rows, int64_t n, int64_t offset, const int64_t* row_off, float* band,
                      void* stream);
 
 /* ---- naive_clusterer.NaiveClusterer (naive_clusterer.py:59-101) ------------------------------

@@ -66,6 +66,8 @@ PROTOTYPES = {
     "sc_diffuse_rowmax_tiles_fold": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_row_stats": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     "sc_affinity_stats": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr],
+    "sc_affinity_stats_rows": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr],
+    "sc_affinity_stats_finish": [c_ptr, c_ptr, c_i64, c_ptr, c_ptr],
     "sc_row_normalize": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64, c_ptr],
     "sc_laplacian": [c_ptr, c_ptr, c_i64, c_i64, c_int, c_dbl, c_ptr, c_i64, c_ptr],
     "sc_affinity_cosine_block": [c_ptr, c_int, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64,
@@ -142,6 +144,9 @@ PROTOTYPES = {
     "sc_complete_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_average_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_gmm_band_pass": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_int, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_gmm_band_pass_packed": [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_int, c_ptr, c_ptr, c_ptr,
+                                c_ptr],
+    "sc_gmm_band_pack": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr],
     "sc_naive_cluster": [c_ptr, c_ptr, c_int, c_i64, c_i64, c_i64, c_dbl, c_dbl, c_i64, c_ptr,
                          c_i64, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
 }

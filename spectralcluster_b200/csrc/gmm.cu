@@ -3,9 +3,13 @@
 // affinity[np.triu_indices(n, offset)], one streaming pass each.  The control flow (KMeans++,
 // Lloyd, EM, BIC) is host logic in spectralcluster_b200/gmm_bic.py.
 //
-// The band of row i is columns [max(0, i + offset), n) of the fp32 [n, lda] matrix; nothing else
-// is read (no padding, no column >= n).  One CTA per row: the ragged head up to the next multiple
-// of 4 is read scalar, the body with 128-bit loads, the tail (n % 4) scalar.  Each sample is
+// The band of row i is columns [j0, n), j0 = max(0, i + offset), of the fp32 [n, lda] matrix;
+// nothing else is read (no padding, no column >= n).  The same passes read a packed band (the
+// factored route, which never stores the matrix): row i's columns [c0, n), c0 = j0 & ~3, at
+// band[row_off[i] ...] with row_off[i] % 4 == 0, so column j keeps its position mod 4 and every
+// thread adds the same samples in the same order as on the dense matrix.  One CTA per row: the
+// ragged head up to the next multiple of 4 is read scalar, the body with 128-bit loads, the tail
+// (n % 4) scalar.  Each sample is
 // promoted to fp64 and every operation and sum is fp64 (exp / log1p included).  Each CTA writes
 // its row's partial sums to `work` (per-thread sequential sums, then the fixed block tree); one
 // block sums the rows in a fixed order, so the result is the same bit for bit on every call.
@@ -126,9 +130,22 @@ struct RowAcc {
   }
 };
 
-template <int MODE>
-__global__ void __launch_bounds__(GT) k_gmm_rows(const float* __restrict__ a, int64_t n,
-                                                 int64_t lda, int64_t offset, GmmArgs g,
+// Row accessors: row(i, j0) points at column 0 of band row i, valid from column j0 & ~3 on.
+struct DenseRows {         // the [n, lda] matrix
+  const float* __restrict__ a;
+  int64_t lda;
+  __device__ __forceinline__ const float* row(int64_t i, int64_t) const { return a + i * lda; }
+};
+struct PackedRows {        // the packed band: columns [c0, n) of row i at band + row_off[i]
+  const float* __restrict__ band;
+  const int64_t* __restrict__ row_off;
+  __device__ __forceinline__ const float* row(int64_t i, int64_t j0) const {
+    return band + (row_off[i] - (j0 & ~(int64_t)3));
+  }
+};
+
+template <int MODE, class Rows>
+__global__ void __launch_bounds__(GT) k_gmm_rows(Rows rows, int64_t n, int64_t offset, GmmArgs g,
                                                  double* __restrict__ part) {
   __shared__ double red[32];
   const int64_t i = blockIdx.x;
@@ -136,7 +153,7 @@ __global__ void __launch_bounds__(GT) k_gmm_rows(const float* __restrict__ a, in
   RowAcc<MODE> acc;
   acc.init();
   if (j0 < n) {
-    const float* r = a + i * lda;
+    const float* r = rows.row(i, j0);
     const int64_t jv = ((j0 + 3) & ~(int64_t)3) < n ? ((j0 + 3) & ~(int64_t)3) : n;
     const int64_t jend = n & ~(int64_t)3;
     for (int64_t j = j0 + threadIdx.x; j < jv; j += GT) acc.add(r[j], g);
@@ -222,8 +239,8 @@ __device__ int64_t scan_count(int64_t len, double base, double target, Term term
 // u * pot of searchsorted(cumsum(d0), target) over the KMeans++ distances to the centre p[1] (centred
 // by p[0]): first over the row sums the preceding SC_GMM_KPP pass left in work[0..n), then inside
 // the row.  Both clip to m - 1.  out[q] = index, out[2 + q] = the sample (fp32 promoted).
-__global__ void __launch_bounds__(GL) k_gmm_lookup(const float* __restrict__ a, int64_t n,
-                                                   int64_t lda, int64_t offset, GmmArgs g,
+template <class Rows>
+__global__ void __launch_bounds__(GL) k_gmm_lookup(Rows band, int64_t n, int64_t offset, GmmArgs g,
                                                    const double* __restrict__ rowsum,
                                                    double* __restrict__ out) {
   __shared__ double chunk[GL];
@@ -245,7 +262,7 @@ __global__ void __launch_bounds__(GL) k_gmm_lookup(const float* __restrict__ a, 
       } else {
         const double base = s_prefix;
         const int64_t j0 = row + offset > 0 ? row + offset : 0;
-        const float* r = a + row * lda + j0;
+        const float* r = band.row(row, j0) + j0;
         const int64_t k = scan_count(n - j0, base, target,
                                      [&](int64_t t) { return sqdist1((double)r[t] - mean, c0); },
                                      chunk, &s_count, &s_prefix);
@@ -261,12 +278,40 @@ __global__ void __launch_bounds__(GL) k_gmm_lookup(const float* __restrict__ a, 
       if (band_start(n, offset, mid) <= idx) lo = mid;
       else hi = mid - 1;
     }
-    const int64_t j = (lo + offset > 0 ? lo + offset : 0) + idx - band_start(n, offset, lo);
+    const int64_t jl = lo + offset > 0 ? lo + offset : 0;
+    const int64_t j = jl + idx - band_start(n, offset, lo);
     if (threadIdx.x == 0) {
       out[q] = (double)idx;
-      out[2 + q] = (double)a[lo * lda + j];
+      out[2 + q] = (double)band.row(lo, jl)[j];
     }
     __syncthreads();
+  }
+}
+
+// Rows [row_begin, row_begin + rows) of an fp32 panel (panel row r = matrix row row_begin + r)
+// -> their packed band rows.  The slots [c0, j0) and [n, round_up(n, 4)) are NaN, so a pass that
+// strays outside the band sums to a non-finite value.  One CTA per row, 128-bit loads and stores
+// (c0, lda and row_off[i] are multiples of 4).
+__global__ void __launch_bounds__(GT) k_gmm_band_pack(const float* __restrict__ panel, int64_t ldp,
+                                                      int64_t row_begin, int64_t n, int64_t offset,
+                                                      const int64_t* __restrict__ row_off,
+                                                      float* __restrict__ band) {
+  const int64_t i = row_begin + blockIdx.x;
+  const int64_t j0 = i + offset > 0 ? i + offset : 0;
+  if (j0 >= n) return;
+  const int64_t c0 = j0 & ~(int64_t)3;
+  const float* r = panel + (int64_t)blockIdx.x * ldp;
+  float* o = band + row_off[i] - c0;
+  const int64_t cend = (n + 3) & ~(int64_t)3;
+  for (int64_t j = c0 + 4 * (int64_t)threadIdx.x; j < cend; j += 4 * GT) {
+    float4 q = ld_stream4(r + j);
+    if (j < j0 || j + 3 >= n) {
+      q.x = (j < j0 || j >= n) ? NAN : q.x;
+      q.y = (j + 1 < j0 || j + 1 >= n) ? NAN : q.y;
+      q.z = (j + 2 < j0 || j + 2 >= n) ? NAN : q.z;
+      q.w = (j + 3 < j0 || j + 3 >= n) ? NAN : q.w;
+    }
+    *reinterpret_cast<float4*>(o + j) = q;
   }
 }
 
@@ -274,22 +319,20 @@ __global__ void __launch_bounds__(GL) k_gmm_lookup(const float* __restrict__ a, 
 
 using namespace sc;
 
-template <int MODE>
-static void launch_rows(const float* a, int64_t n, int64_t lda, int64_t offset, const GmmArgs& g,
-                        double* part, cudaStream_t st) {
-  k_gmm_rows<MODE><<<(unsigned)n, GT, 0, st>>>(a, n, lda, offset, g, part);
+template <int MODE, class Rows>
+static void launch_rows(Rows rows, int64_t n, int64_t offset, const GmmArgs& g, double* part,
+                        cudaStream_t st) {
+  k_gmm_rows<MODE><<<(unsigned)n, GT, 0, st>>>(rows, n, offset, g, part);
   sc::launched();
 }
 
-extern "C" int sc_gmm_band_pass(sc_context* ctx, const float* a, int64_t n, int64_t lda,
-                                int64_t offset, int mode, const double* params_host, double* work,
-                                double* out_host, void* stream) {
-  SC_REQUIRE(ctx && a && params_host && work && out_host && n > 0 && lda >= n,
-             "sc_gmm_band_pass: bad arguments");
-  SC_REQUIRE(vec_ok_f32(a, lda), "sc_gmm_band_pass: `a` needs a 16-byte aligned base and lda %% 4 == 0");
-  SC_REQUIRE(offset < n - 1, "sc_gmm_band_pass: offset must be below n - 1");
-  SC_REQUIRE(n < (int64_t)1 << 31, "sc_gmm_band_pass: n too large");
-  SC_REQUIRE(mode >= SC_GMM_MOMENTS && mode <= SC_GMM_SCORE, "sc_gmm_band_pass: unknown mode %d", mode);
+// One pass of `mode` over the band behind `rows` (sc_gmm_band_pass, sc_gmm_band_pass_packed).
+template <class Rows>
+static int band_pass(const char* name, Rows rows, int64_t n, int64_t offset, int mode,
+                     const double* params_host, double* work, double* out_host, void* stream) {
+  SC_REQUIRE(offset < n - 1, "%s: offset must be below n - 1", name);
+  SC_REQUIRE(n < (int64_t)1 << 31, "%s: n too large", name);
+  SC_REQUIRE(mode >= SC_GMM_MOMENTS && mode <= SC_GMM_SCORE, "%s: unknown mode %d", name, mode);
   cudaStream_t st = as_stream(stream);
   GmmArgs g;
   for (int k = 0; k < 16; ++k) g.p[k] = params_host[k];
@@ -298,22 +341,59 @@ extern "C" int sc_gmm_band_pass(sc_context* ctx, const float* a, int64_t n, int6
     if (g.p[2] == 0.0) {
       const double m = (double)band_start(n, offset, n);
       SC_REQUIRE(g.p[3] >= 0.0 && g.p[3] < m && g.p[4] >= 0.0 && g.p[4] < m,
-                 "sc_gmm_band_pass: lookup index out of range");
+                 "%s: lookup index out of range", name);
     }
-    k_gmm_lookup<<<1, GL, 0, st>>>(a, n, lda, offset, g, work, out_dev); sc::launched();
+    k_gmm_lookup<<<1, GL, 0, st>>>(rows, n, offset, g, work, out_dev); sc::launched();
   } else {
     switch (mode) {
-      case SC_GMM_MOMENTS: launch_rows<SC_GMM_MOMENTS>(a, n, lda, offset, g, work, st); break;
-      case SC_GMM_KPP: launch_rows<SC_GMM_KPP>(a, n, lda, offset, g, work, st); break;
-      case SC_GMM_LLOYD: launch_rows<SC_GMM_LLOYD>(a, n, lda, offset, g, work, st); break;
-      case SC_GMM_LABELS: launch_rows<SC_GMM_LABELS>(a, n, lda, offset, g, work, st); break;
-      case SC_GMM_EM: launch_rows<SC_GMM_EM>(a, n, lda, offset, g, work, st); break;
-      default: launch_rows<SC_GMM_SCORE>(a, n, lda, offset, g, work, st); break;
+      case SC_GMM_MOMENTS: launch_rows<SC_GMM_MOMENTS>(rows, n, offset, g, work, st); break;
+      case SC_GMM_KPP: launch_rows<SC_GMM_KPP>(rows, n, offset, g, work, st); break;
+      case SC_GMM_LLOYD: launch_rows<SC_GMM_LLOYD>(rows, n, offset, g, work, st); break;
+      case SC_GMM_LABELS: launch_rows<SC_GMM_LABELS>(rows, n, offset, g, work, st); break;
+      case SC_GMM_EM: launch_rows<SC_GMM_EM>(rows, n, offset, g, work, st); break;
+      default: launch_rows<SC_GMM_SCORE>(rows, n, offset, g, work, st); break;
     }
     k_gmm_finish<<<1, 1024, 0, st>>>(work, n, mode, out_dev); sc::launched();
   }
   SC_LAUNCH_CHECK();
   SC_CUDA(cudaMemcpyAsync(out_host, out_dev, sizeof(double) * GF, cudaMemcpyDeviceToHost, st));
   SC_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+extern "C" int sc_gmm_band_pass(sc_context* ctx, const float* a, int64_t n, int64_t lda,
+                                int64_t offset, int mode, const double* params_host, double* work,
+                                double* out_host, void* stream) {
+  SC_REQUIRE(ctx && a && params_host && work && out_host && n > 0 && lda >= n,
+             "sc_gmm_band_pass: bad arguments");
+  SC_REQUIRE(vec_ok_f32(a, lda), "sc_gmm_band_pass: `a` needs a 16-byte aligned base and lda %% 4 == 0");
+  return band_pass("sc_gmm_band_pass", DenseRows{a, lda}, n, offset, mode, params_host, work,
+                   out_host, stream);
+}
+
+extern "C" int sc_gmm_band_pass_packed(sc_context* ctx, const float* band, const int64_t* row_off,
+                                       int64_t n, int64_t offset, int mode,
+                                       const double* params_host, double* work, double* out_host,
+                                       void* stream) {
+  SC_REQUIRE(ctx && band && row_off && params_host && work && out_host && n > 0,
+             "sc_gmm_band_pass_packed: bad arguments");
+  SC_REQUIRE(vec_ok_f32(band, 0), "sc_gmm_band_pass_packed: `band` needs a 16-byte aligned base");
+  return band_pass("sc_gmm_band_pass_packed", PackedRows{band, row_off}, n, offset, mode,
+                   params_host, work, out_host, stream);
+}
+
+extern "C" int sc_gmm_band_pack(sc_context* ctx, const float* panel, int64_t ldp, int64_t row_begin,
+                                int64_t rows, int64_t n, int64_t offset, const int64_t* row_off,
+                                float* band, void* stream) {
+  SC_REQUIRE(ctx && panel && row_off && band && n > 0 && rows > 0 && row_begin >= 0 &&
+             row_begin + rows <= n && ldp >= ((n + 3) & ~(int64_t)3),
+             "sc_gmm_band_pack: bad arguments");
+  SC_REQUIRE(vec_ok_f32(panel, ldp), "sc_gmm_band_pack: `panel` needs a 16-byte aligned base and ldp %% 4 == 0");
+  SC_REQUIRE(vec_ok_f32(band, 0), "sc_gmm_band_pack: `band` needs a 16-byte aligned base");
+  SC_REQUIRE(offset < n - 1, "sc_gmm_band_pack: offset must be below n - 1");
+  k_gmm_band_pack<<<(unsigned)rows, GT, 0, as_stream(stream)>>>(panel, ldp, row_begin, n, offset,
+                                                                row_off, band);
+  sc::launched();
+  SC_LAUNCH_CHECK();
   return 0;
 }

@@ -349,12 +349,15 @@ __global__ void k_gather_rows_f16(const __half* __restrict__ src, int64_t lds,
 // fallback_clusterer.check_single_cluster (fallback_clusterer.py:127-187) needs three reductions
 // of the affinity: its minimum (AllAffinity, :143), the minimum of the first super-diagonal
 // (NeighborAffinity, :148-150) and np.std over all n^2 entries (AffinityStd, :154).  One
-// streaming pass, fp64 accumulation; per-row partials, then a single-block finish.
+// streaming pass, fp64 accumulation; per-row partials, then a single-block finish.  The factored
+// route, which never stores the affinity, runs the same row kernel over row panels: a panel's row r
+// is matrix row row_begin + r, and with `nb` each row also records a[i][i+1] for the finish.
 __global__ void k_affinity_row_stats(const float* __restrict__ a, int64_t n, int64_t lda,
-                                     double* __restrict__ part /*[3][n]*/) {
+                                     int64_t row_begin, double* __restrict__ part /*[3][n]*/,
+                                     double* __restrict__ nb /*[n] or null*/) {
   __shared__ double red[32];
-  const int64_t i = blockIdx.x;
-  const float* r = a + i * lda;
+  const int64_t i = row_begin + blockIdx.x;
+  const float* r = a + (int64_t)blockIdx.x * lda;
   double mn = INFINITY, s = 0.0, q2 = 0.0;
   const int64_t n4 = n & ~(int64_t)3;
   for (int64_t j = (int64_t)threadIdx.x * 4; j < n4; j += (int64_t)blockDim.x * 4) {
@@ -376,10 +379,12 @@ __global__ void k_affinity_row_stats(const float* __restrict__ a, int64_t n, int
     part[i] = mn;
     part[n + i] = s;
     part[2 * n + i] = q2;
+    if (nb) nb[i] = i + 1 < n ? (double)r[i + 1] : INFINITY;
   }
 }
 
-// out[0] = min, out[1] = sum, out[2] = sum of squares, out[3] = min_i a[i][i+1] (+inf if n == 1)
+// out[0] = min, out[1] = sum, out[2] = sum of squares, out[3] = min_i a[i][i+1] (+inf if n == 1),
+// the neighbours read from `a` or, with a == null, from the row kernel's part[3 n + i]
 __global__ void k_affinity_stats_finish(const double* __restrict__ part, const float* __restrict__ a,
                                         int64_t n, int64_t lda, double* __restrict__ out) {
   __shared__ double red[32];
@@ -388,7 +393,7 @@ __global__ void k_affinity_stats_finish(const double* __restrict__ part, const f
     mn = fmin(mn, part[i]);
     s += part[n + i];
     q2 += part[2 * n + i];
-    if (i + 1 < n) nb = fmin(nb, (double)a[i * lda + i + 1]);
+    if (i + 1 < n) nb = fmin(nb, a ? (double)a[i * lda + i + 1] : part[3 * n + i]);
   }
   mn = -block_maxd(-mn, red);
   s = block_sum(s, red);
@@ -599,10 +604,34 @@ extern "C" int sc_affinity_stats(sc_context* ctx, const float* a, int64_t n, int
   Scratch part;
   SC_CUDA(part.alloc(sizeof(double) * (size_t)(3 * n + 4), st));
   double* p = part.as<double>();
-  k_affinity_row_stats<<<(unsigned)n, 256, 0, st>>>(a, n, lda, p); sc::launched();
+  k_affinity_row_stats<<<(unsigned)n, 256, 0, st>>>(a, n, lda, 0, p, nullptr); sc::launched();
   k_affinity_stats_finish<<<1, 1024, 0, st>>>(p, a, n, lda, p + 3 * n); sc::launched();
   SC_LAUNCH_CHECK();
   SC_CUDA(cudaMemcpyAsync(out_host, p + 3 * n, sizeof(double) * 4, cudaMemcpyDeviceToHost, st));
+  SC_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+extern "C" int sc_affinity_stats_rows(sc_context* ctx, const float* panel, int64_t rows, int64_t n,
+                                      int64_t ldp, int64_t row_begin, double* part, void* stream) {
+  SC_REQUIRE(ctx && panel && part && n > 0 && rows > 0 && row_begin >= 0 && row_begin + rows <= n &&
+             ldp >= n, "sc_affinity_stats_rows: bad arguments");
+  SC_REQUIRE(vec_ok_f32(panel, ldp),
+             "sc_affinity_stats_rows: `panel` needs a 16-byte aligned base and ldp %% 4 == 0");
+  k_affinity_row_stats<<<(unsigned)rows, 256, 0, as_stream(stream)>>>(panel, n, ldp, row_begin,
+                                                                       part, part + 3 * n);
+  sc::launched();
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int sc_affinity_stats_finish(sc_context* ctx, double* part, int64_t n, double* out_host,
+                                        void* stream) {
+  SC_REQUIRE(ctx && part && out_host && n > 0, "sc_affinity_stats_finish: bad arguments");
+  cudaStream_t st = as_stream(stream);
+  k_affinity_stats_finish<<<1, 1024, 0, st>>>(part, nullptr, n, 0, part + 4 * n); sc::launched();
+  SC_LAUNCH_CHECK();
+  SC_CUDA(cudaMemcpyAsync(out_host, part + 4 * n, sizeof(double) * 4, cudaMemcpyDeviceToHost, st));
   SC_CUDA(cudaStreamSynchronize(st));
   return 0;
 }

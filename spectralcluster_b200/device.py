@@ -248,7 +248,11 @@ class Engine:
       "sc_eigh_mapback": "utils.compute_sorted_eigenvectors",
       "sc_kmeans": "custom_distance_kmeans.run_kmeans", "sc_row_renorm": "spectral_clusterer.row_wise_renorm",
       "sc_affinity_stats": "fallback_clusterer.check_single_cluster",
+      "sc_affinity_stats_rows": "fallback_clusterer.check_single_cluster",
+      "sc_affinity_stats_finish": "fallback_clusterer.check_single_cluster",
       "sc_gmm_band_pass": "fallback_clusterer.check_single_cluster",
+      "sc_gmm_band_pass_packed": "fallback_clusterer.check_single_cluster",
+      "sc_gmm_band_pack": "fallback_clusterer.check_single_cluster",
       "sc_constraint_combine": "constraint.adjust_affinity", "sc_scale_shift": "constraint.adjust_affinity",
       "sc_normalize_rows_typed": "utils.compute_affinity_matrix",
       "sc_cluster_centroids": "utils.get_cluster_centroids",
@@ -831,6 +835,46 @@ class FactoredAffinity:
       panel = eng.affinity_panel(self.hi, self.lo, self.n, self.d, a0, a1, diag)
       yield r0, r1, panel, a0, diag, b
       del panel
+
+  def _rows(self, eng: Engine, stop: typing.Optional[int] = None):
+    """Yield (r0, r1, affinity rows [r0, r1)) over panel_plan(), without the blur halo, for the
+    panels that start below `stop`."""
+    for r0, r1, _, _ in panel_plan(self.n, self.panel_rows):
+      if stop is not None and r0 >= stop:
+        break
+      panel = eng.affinity_panel(self.hi, self.lo, self.n, self.d, r0, r1)
+      yield r0, r1, panel
+      del panel
+
+  def statistics(self, eng: Engine) -> typing.Dict[str, float]:
+    """{min, neighbor_min, std} of the affinity for the single-cluster checks: the per-row partials
+    of sc_affinity_stats over one sweep of row panels, finished in its order, so the values are
+    those of the stored affinity bit for bit."""
+    n = self.n
+    part = eng.vector(4 * n + 4)
+    for r0, r1, panel in self._rows(eng):
+      eng.call("sc_affinity_stats_rows", _ptr(panel), r1 - r0, n, panel.stride(0), r0, _ptr(part),
+               eng.stream)
+    from . import fallback_clusterer
+    out = np.zeros(4, dtype=np.float64)
+    eng.call("sc_affinity_stats_finish", _ptr(part), n, out.ctypes.data_as(ctypes.c_void_p),
+             eng.stream)
+    return fallback_clusterer.statistics_from_sums(out, n)
+
+  def upper_band(self, eng: Engine, offset: int):
+    """(band, row_off): the packed band affinity[np.triu_indices(n, offset)] of the AffinityGmmBic
+    check (gmm_bic.packed_row_offsets; fp32, NaN in its padding slots) and its device row offsets,
+    from one sweep of row panels."""
+    from . import gmm_bic
+    t = torch()
+    n = self.n
+    off = gmm_bic.packed_row_offsets(n, offset)
+    band = t.empty((max(int(off[-1]), 4),), dtype=t.float32, device=eng.device)
+    row_off = t.from_numpy(off).to(eng.device)
+    for r0, r1, panel in self._rows(eng, stop=gmm_bic.band_rows(n, offset)):
+      eng.call("sc_gmm_band_pack", _ptr(panel), panel.stride(0), r0, r1 - r0, n, int(offset),
+               _ptr(row_off), _ptr(band), eng.stream)
+    return band, row_off
 
   def rowmax(self, eng: Engine, options):
     """m of the symmetric blur pair (pass 1 over every panel), computed once."""

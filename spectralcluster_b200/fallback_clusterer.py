@@ -4,11 +4,15 @@
 
 What runs where:
   * AllAffinity / NeighborAffinity / AffinityStd are reductions over the N x N affinity: one
-    streaming pass on the device (`sc_affinity_stats`), four doubles come back;
+    streaming pass on the device (`sc_affinity_stats`), four doubles come back; on the factored
+    route, whose affinity is never stored, one sweep of affinity row panels
+    (FactoredAffinity.statistics) gives the same four doubles bit for bit;
   * AffinityGmmBic fits 1- and 2-component GMMs to the N^2/2 upper-band affinities: on the
     device for a device-resident affinity, one streaming pass per KMeans / EM step
-    (`gmm_bic`, `sc_gmm_band_pass`), with scikit-learn's arithmetic and random draws; a host
-    ndarray still goes to scikit-learn;
+    (`gmm_bic`, `sc_gmm_band_pass`), with scikit-learn's arithmetic and random draws; on the
+    factored route over the packed band (FactoredAffinity.upper_band, `sc_gmm_band_pass_packed`),
+    with the same sums bit for bit, held only while the check runs; a host ndarray still goes to
+    scikit-learn;
   * FallbackClusterer as the probe of predict(), Agglomerative type: average-linkage cosine AHC
     on the device with scikit-learn's cluster count (agglomerative.CosineAverageLinkage); a host
     ndarray affinity still goes to scikit-learn;
@@ -90,7 +94,8 @@ class FallbackClusterer:
 
 
 def affinity_statistics(affinity) -> typing.Dict[str, float]:
-  """{min, neighbor_min, std} of a host ndarray or a device-resident affinity."""
+  """{min, neighbor_min, std} of a host ndarray, a device-resident affinity or the FactoredAffinity
+  of the factored route."""
   if isinstance(affinity, np.ndarray):
     return dict(min=float(affinity.min()),
                 neighbor_min=float(np.diag(affinity, k=1).min()) if affinity.shape[0] > 1 else np.inf,
@@ -98,10 +103,17 @@ def affinity_statistics(affinity) -> typing.Dict[str, float]:
   import ctypes
   from . import device as dev
   eng = dev.Engine.get()
+  if isinstance(affinity, dev.FactoredAffinity):
+    return affinity.statistics(eng)
   out = np.zeros(4, dtype=np.float64)
   n = affinity.n
   eng.call("sc_affinity_stats", dev._ptr(affinity.matrix), n, affinity.matrix.stride(0),
            out.ctypes.data_as(ctypes.c_void_p), eng.stream)
+  return statistics_from_sums(out, n)
+
+
+def statistics_from_sums(out, n: int) -> typing.Dict[str, float]:
+  """{min, neighbor_min, std} from sc_affinity_stats's (min, sum, sum of squares, neighbour min)."""
   count = float(n) * float(n)
   mean = out[1] / count
   var = max(out[2] / count - mean * mean, 0.0)
@@ -114,7 +126,8 @@ def check_single_cluster(fallback_options: FallbackOptions,
                          embeddings_dev=None) -> bool:
   """True when the data form a single cluster (only consulted when min_clusters == 1).
 
-  `affinity` is a host ndarray (reference signature) or the DeviceAffinity predict() holds.
+  `affinity` is a host ndarray (reference signature), or the DeviceAffinity or FactoredAffinity
+  predict() holds; the two device forms give the same verdict and `details`, bit for bit.
   For AffinityGmmBic on a device affinity, `details` (if given) receives the two BICs, both
   GMMs' EM iteration counts and the number of passes over the affinity.  Both fallback clusterer
   types on a device affinity run on the device too, on `embeddings_dev` (the embeddings as a CUDA
@@ -138,7 +151,14 @@ def check_single_cluster(fallback_options: FallbackOptions,
     if not isinstance(affinity, np.ndarray):
       from . import device as dev
       from . import gmm_bic
-      res = gmm_bic.gmm_bic(gmm_bic.DeviceOps(dev.Engine.get(), affinity.matrix, n, offset))
+      eng = dev.Engine.get()
+      if isinstance(affinity, dev.FactoredAffinity):
+        # the packed band lives only for the check: refine() allocates Y_hi after it is freed
+        band, row_off = affinity.upper_band(eng, offset)
+        res = gmm_bic.gmm_bic(gmm_bic.DeviceOps(eng, band, n, offset, row_off))
+        del band, row_off
+      else:
+        res = gmm_bic.gmm_bic(gmm_bic.DeviceOps(eng, affinity.matrix, n, offset))
       if details is not None:
         details.update(bic=res.bic, n_iter=res.n_iter, passes=res.passes)
       return res.single

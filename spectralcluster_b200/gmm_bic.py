@@ -26,7 +26,9 @@ moved to the mean exactly: sum r (x - mu)^2 = Q - 2 (mu - s) (R1 - s R0) + (mu -
 
 `NumpyOps` evaluates each reduction on a host copy of the band with NumPy in scikit-learn's order
 (the CPU tests compare the recurrence with scikit-learn itself); `DeviceOps` calls
-`sc_gmm_band_pass`, one streaming pass over the fp32 device matrix.
+`sc_gmm_band_pass`, one streaming pass over the fp32 device matrix, or `sc_gmm_band_pass_packed`
+over the packed band (`packed_row_offsets`) of an affinity that is never stored; both return the
+same sums bit for bit.
 """
 
 from __future__ import annotations
@@ -79,6 +81,18 @@ def band_position(n: int, offset: int, idx: int):
     else:
       hi = mid - 1
   return lo, max(0, lo + offset) + idx - band_start(n, offset, lo)
+
+
+def packed_row_offsets(n: int, offset: int) -> np.ndarray:
+  """row_off [n + 1] (int64) of the packed band: row i (j0 = max(0, i + offset) < n) keeps columns
+  [c0, n), c0 = j0 & ~3, at band[row_off[i] ...], padded to a multiple of 4 so that column j sits
+  at the position mod 4 it has in a dense matrix with ld % 4 == 0; rows without band elements take
+  no room.  row_off[n] is the packed length in elements."""
+  j0 = np.maximum(np.arange(n, dtype=np.int64) + offset, 0)
+  width = np.where(j0 < n, (n - (j0 & ~3) + 3) & ~3, 0)
+  out = np.zeros(n + 1, dtype=np.int64)
+  np.cumsum(width, out=out[1:])
+  return out
 
 
 # ---- RandomState.choice(m, p=uniform) without m values ------------------------------------------
@@ -377,11 +391,14 @@ class NumpyOps:
 
 class DeviceOps:
   """CUDA backend: each reduction is one `sc_gmm_band_pass` over the fp32 device matrix
-  [n, lda]; only the band j >= max(0, i + offset), j < n is read."""
+  [n, lda]; only the band j >= max(0, i + offset), j < n is read.  With `row_off` (the device copy
+  of packed_row_offsets(n, offset)), `matrix` is the packed band and each reduction is one
+  `sc_gmm_band_pass_packed`."""
 
-  def __init__(self, eng, matrix, n, offset):
+  def __init__(self, eng, matrix, n, offset, row_off=None):
     from . import device as dev
     self.eng, self.a, self.n, self.offset = eng, matrix, int(n), int(offset)
+    self.row_off = row_off
     self.m = band_size(self.n, self.offset)
     self.ptr = dev._ptr
     # per-row partials of up to 8 fields; the KMeans++ row sums stay here for the lookup
@@ -395,9 +412,14 @@ class DeviceOps:
     self.passes += 1
     self.params[:] = 0.0
     self.params[:len(params)] = params
-    self.eng.call("sc_gmm_band_pass", self.ptr(self.a), self.n, self.a.stride(0), self.offset,
-                  mode, self.params.ctypes.data_as(ctypes.c_void_p), self.ptr(self.work),
-                  self.out.ctypes.data_as(ctypes.c_void_p), self.eng.stream)
+    tail = (self.params.ctypes.data_as(ctypes.c_void_p), self.ptr(self.work),
+            self.out.ctypes.data_as(ctypes.c_void_p), self.eng.stream)
+    if self.row_off is None:
+      self.eng.call("sc_gmm_band_pass", self.ptr(self.a), self.n, self.a.stride(0), self.offset,
+                    mode, *tail)
+    else:
+      self.eng.call("sc_gmm_band_pass_packed", self.ptr(self.a), self.ptr(self.row_off), self.n,
+                    self.offset, mode, *tail)
     return self.out
 
   def moments(self, shift):

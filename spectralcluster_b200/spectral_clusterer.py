@@ -230,42 +230,55 @@ class SpectralClusterer:
       self.last_details["diffuse"] = dict(tiles=computed, of=total, operator="factored")
     return w, v, k, gap
 
-  def _operator_scope(self, eng, n: int, constraint_matrix=None) -> bool:
+  def _operator_scope(self, eng, n: int, constraint_matrix=None, single_check=False) -> bool:
     """The options every route that never stores S serves: the default affinity, the fused chain
     closed by a single-MMA Diffuse (dev.factored_sequence_ok), no constraint, min_clusters != 1 and
-    no autotune_group."""
+    no autotune_group.  `single_check`: min_clusters == 1 is served too (the factored route's
+    single-cluster check, _factored_single_cluster_route)."""
     return (self.affinity_function is utils.compute_affinity_matrix and
-            self.min_clusters != 1 and
+            (self.min_clusters != 1 or single_check) and
             not (self.constraint_options and constraint_matrix is not None) and
             self.autotune_group is None and
             dev.factored_sequence_ok(eng, self.refinement_options) and
             eng.gemm_engine(n) == nat.GEMM_TCGEN05 and
             eng.diffuse_precision_for(n) == nat.GEMM_SINGLE)
 
-  def _lanczos_scope(self, eng, n: int, constraint_matrix=None) -> bool:
+  def _lanczos_scope(self, eng, n: int, constraint_matrix=None, single_check=False) -> bool:
     """The calls of _operator_scope that one Lanczos solve serves (bounded max_clusters <
     LANCZOS_MAX_PAIRS that lanczos_fits): those of the two one-solve routes below."""
     limit = (self.max_clusters or 0) + 1
     return (self.max_clusters is not None and self.max_clusters < LANCZOS_MAX_PAIRS and
             (self.min_clusters or 0) <= limit and
             n > limit and n > eng.dense_eig_max and lanczos_fits(n, limit) and
-            self._operator_scope(eng, n, constraint_matrix))
+            self._operator_scope(eng, n, constraint_matrix, single_check))
 
-  def _factored_route(self, eng, n: int, constraint_matrix=None) -> bool:
+  def _factored_route(self, eng, n: int, constraint_matrix=None, single_check=False) -> bool:
     """Whether predict() on n embeddings takes the factored route with one Lanczos solve: the
     stored route's peak (computed from shapes) exceeds eng.factored_above_bytes and every option
     is one _lanczos_scope accepts.  _factored_windows_route covers the eigen options one solve
-    cannot serve; any other call keeps the stored route."""
-    return (self._lanczos_scope(eng, n, constraint_matrix) and
+    cannot serve, _factored_single_cluster_route the calls with min_clusters == 1; any other call
+    keeps the stored route."""
+    return (self._lanczos_scope(eng, n, constraint_matrix, single_check) and
             dev.stored_route_peak_bytes(n) > eng.factored_above_bytes)
 
-  def _factored_windows_route(self, eng, n: int, constraint_matrix=None) -> bool:
+  def _factored_windows_route(self, eng, n: int, constraint_matrix=None,
+                              single_check=False) -> bool:
     """Whether predict() on n embeddings takes the factored route with the windowed solve
     (eigen_windows.py on the factored operator): as _factored_route, but for max_clusters=None or
     more pairs than one Lanczos solve finds.  Disjoint from _factored_route."""
     return ((self.max_clusters is None or self.max_clusters + 1 > LANCZOS_MAX_PAIRS) and
             n > DENSE_MAX_N and dev.stored_route_peak_bytes(n) > eng.factored_above_bytes and
-            self._operator_scope(eng, n, constraint_matrix))
+            self._operator_scope(eng, n, constraint_matrix, single_check))
+
+  def _factored_single_cluster_route(self, eng, n: int, constraint_matrix=None) -> bool:
+    """Whether predict() on n embeddings with min_clusters == 1 takes the factored route: the calls
+    _factored_route or _factored_windows_route would take if min_clusters were not 1.  The
+    single-cluster check runs on panels of the affinity (FactoredAffinity.statistics /
+    upper_band), then the eigen stage as on those routes.  Disjoint from the other three routes,
+    which refuse min_clusters == 1."""
+    return self.min_clusters == 1 and (
+        self._factored_route(eng, n, constraint_matrix, single_check=True) or
+        self._factored_windows_route(eng, n, constraint_matrix, single_check=True))
 
   def _bounded_route(self, eng, n: int, constraint_matrix=None) -> bool:
     """Whether the stored front end (a resident affinity) replaces the storing Diffuse and the
@@ -374,7 +387,8 @@ class SpectralClusterer:
         x = x.astype(np.float64)
       x_dev = t.from_numpy(x).to(eng.device, non_blocking=True)
     if (self._factored_route(eng, num_embeddings, constraint_matrix) or
-        self._factored_windows_route(eng, num_embeddings, constraint_matrix)):
+        self._factored_windows_route(eng, num_embeddings, constraint_matrix) or
+        self._factored_single_cluster_route(eng, num_embeddings, constraint_matrix)):
       affinity = dev.FactoredAffinity(eng, x_dev)
     elif builtin:
       crop_first = bool(sequence) and sequence[0] == RefinementName.CropDiagonal
@@ -390,7 +404,8 @@ class SpectralClusterer:
 
     single_details = {}
     if self.min_clusters == 1:
-      # single-vs-multi cluster decision on the resident affinity (spectral_clusterer.py:253-256)
+      # single-vs-multi cluster decision (spectral_clusterer.py:253-256) on the resident affinity,
+      # or on affinity panels and the packed upper band on the factored route
       if fallback_clusterer.check_single_cluster(self.fallback_options,
                                                  None if on_device else embeddings, affinity,
                                                  single_details, embeddings_dev=x_dev):
