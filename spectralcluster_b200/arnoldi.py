@@ -24,6 +24,7 @@ class Result:
     self.values = values                # complex Ritz values, ordered (wanted end first)
     self.basis_size = basis_size        # P: the Ritz vectors are V[:P] @ coefficients
     self.coefficients = coefficients    # complex [P, n_values]
+    # restarts counts the locking restarts too
     self.matvecs, self.restarts, self.converged = matvecs, restarts, converged
 
 
@@ -49,9 +50,32 @@ def krylov_schur(ops, n: int, n_values: int, tol: float = 1e-9, basis: int = 0,
     _, nrm2 = ops.orthogonalize(j)
     ops.store(j, 1.0 / np.sqrt(nrm2))
 
+  def schur_keep(hm, theta, keep, ref):
+    """Ordered real Schur form of hm whose leading block holds the `keep` Ritz values of largest
+    real part, more if the cut would split a conjugate pair (or a tie)."""
+    import scipy.linalg
+    p = hm.shape[0]
+    re_sorted = np.sort(theta.real)[::-1]
+    while keep < p - 1 and abs(re_sorted[keep - 1] - re_sorted[keep]) <= 1e-14 * ref:
+      keep += 1                                        # never split a conjugate pair
+    cut = 0.5 * (re_sorted[keep - 1] + re_sorted[keep])
+    t, q, sdim = scipy.linalg.schur(hm, output="real", sort=lambda re, im: re > cut)
+    if sdim < 1 or sdim >= p:
+      raise RuntimeError("krylov_schur: Schur reordering kept %d of %d" % (sdim, p))
+    return t, q, sdim
+
   fresh(0)
   p, matvecs, restarts, converged = 0, 0, 0, 0
   values = coeffs = None
+  # Locking.  One start vector sees a single copy of a repeated eigenvalue in exact arithmetic;
+  # rounding seeds the other copies only slowly, so the wanted set can converge without them.
+  # Once it has converged, its Schur vectors are locked: their residual coupling (each Ritz
+  # vector's share of it within the tolerance) is dropped from H and kept in `drop`, one row per
+  # lock in the coordinates of the current basis, and the basis continues from a fresh random
+  # vector orthogonal to them, i.e. Arnoldi on the complement.  A copy that was missing enters the
+  # wanted set there; the solve ends when such a pass adds nothing to it.  A Ritz pair (theta, V z)
+  # has the residual |coupling z[p-1]| + sum_l |drop_l . z|.
+  drop, probed = np.zeros((0, m)), None
   while True:
     j = p
     while j < m:
@@ -77,7 +101,7 @@ def krylov_schur(ops, n: int, n_values: int, tol: float = 1e-9, basis: int = 0,
     order = np.argsort(-theta.real, kind="stable")
     theta, z = theta[order], z[:, order]
     coupling = h[p, p - 1] if p < n else 0.0           # residual_i = |coupling * z[p-1, i]|
-    resid = np.abs(coupling * z[p - 1, :])
+    resid = np.abs(coupling * z[p - 1, :]) + np.abs(drop[:, :p] @ z).sum(axis=0)
     ref = max(float(np.abs(theta).max()), 1e-300)
     converged = 0
     for i in range(min(n_values, p)):
@@ -86,23 +110,29 @@ def krylov_schur(ops, n: int, n_values: int, tol: float = 1e-9, basis: int = 0,
       else:
         break
     values, coeffs = theta[:n_values], z[:, :n_values]
-    if converged >= min(n_values, p) or p >= n or matvecs >= max_matvecs:
+    done = converged >= min(n_values, p)
+    if p >= n or matvecs >= max_matvecs:
       break
-    # ---- thick restart: ordered real Schur form, keep the leading block
-    import scipy.linalg
-    keep = min(p - 2, n_values + max(8, n_values // 2))
-    re_sorted = np.sort(theta.real)[::-1]
-    while keep < p - 1 and abs(re_sorted[keep - 1] - re_sorted[keep]) <= 1e-14 * ref:
-      keep += 1                                        # never split a conjugate pair
-    cut = 0.5 * (re_sorted[keep - 1] + re_sorted[keep])
-    t, q, sdim = scipy.linalg.schur(hm, output="real", sort=lambda re, im: re > cut)
-    if sdim < 1 or sdim >= p:
-      raise RuntimeError("krylov_schur: Schur reordering kept %d of %d" % (sdim, p))
+    if done and (probed is not None and values[-1].real <= probed + tol * ref or
+                 theta[-1].real >= values[-1].real - 1e-14 * ref):
+      break            # the locked pass found nothing new, or nothing else is there to find
+    # ---- thick restart (or, once converged, locking): ordered real Schur form, keep the
+    # leading block
+    keep = n_values if done else min(p - 2, n_values + max(8, n_values // 2))
+    t, q, sdim = schur_keep(hm, theta, keep, ref)
     row = coupling * q[p - 1, :sdim]
     ops.rotate(np.ascontiguousarray(q[:, :sdim]), p)
+    kept = drop[:, :p] @ q[:, :sdim]
+    drop = np.zeros((len(kept) + done, m))
+    drop[:len(kept), :sdim] = kept
     h[:, :] = 0.0
     h[:sdim, :sdim] = t[:sdim, :sdim]
-    h[sdim, :sdim] = row
+    if done:
+      drop[-1, :sdim] = row
+      probed = values[-1].real
+      fresh(sdim)
+    else:
+      h[sdim, :sdim] = row
     p = sdim
     restarts += 1
   return Result(values, p, coeffs, matvecs, restarts, converged)
