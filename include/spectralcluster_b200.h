@@ -135,13 +135,16 @@ int sc_blur_threshold_symmetrize(sc_context* ctx, const float* a, int64_t n, int
                                  int sym_type, float* y, int64_t ldy, void* hi, void* lo,
                                  int64_t ldh, void* stream);
 
-/* The same chain for a SYMMETRIC whole matrix with the blur evaluated once, on the tiles that touch
- * the upper triangle only (blur(a) is symmetric): sc_blur_upper_rowmax stores those tiles of
- * b = blur(a) (the rest of b is left untouched) and assembles rowmax[i] = max_j b[i,j] from their row
- * and column maxima (zero-fills rowmax itself); sc_threshold_symmetrize_upper then writes the whole
- * y (fp32 and/or planes; lo may be NULL when only the hi plane is wanted, i.e. for a single-MMA
- * Diffuse), mirroring every tile.  10 B (8 B without lo) of HBM traffic per matrix element instead
- * of 12, half the filter arithmetic.  Radius-4 blur only (int(4*sigma+0.5) == 4). */
+/* The same chain for a SYMMETRIC whole matrix with the blur evaluated on the tiles that touch the
+ * upper triangle only (blur(a) is symmetric): sc_blur_upper_rowmax assembles rowmax[i] =
+ * max_j b[i,j], b = blur(a), from the row and column maxima of those tiles (zero-fills rowmax
+ * itself).  With b_out it also stores those tiles of b (the rest of b_out is left untouched) and
+ * sc_threshold_symmetrize_upper writes the whole y from them (fp32 and/or planes; lo may be NULL
+ * when only the hi plane is wanted, i.e. for a single-MMA Diffuse), mirroring every tile.  With
+ * b_out == NULL nothing but rowmax is written, and sc_blur_threshold_symmetrize_upper blurs the
+ * upper triangle of a again and writes y and its mirror -- bit for bit the same y, with no b in
+ * memory: 2 + 2 + 2 B of HBM traffic per matrix element for the hi plane alone.  Radius-4 blur
+ * only (int(4*sigma+0.5) == 4). */
 int sc_blur_upper_rowmax(sc_context* ctx, const float* a, int64_t n, int64_t lda,
                          const float* diag_override, double sigma, int zero_diagonal, float* b_out,
                          int64_t ldb, float* rowmax_out, void* stream);
@@ -149,6 +152,11 @@ int sc_threshold_symmetrize_upper(sc_context* ctx, const float* b, int64_t n, in
                                   const float* rowmax, double p, double mult, int binarize,
                                   int preserve_diagonal, int sym_type, float* y, int64_t ldy,
                                   void* hi, void* lo, int64_t ldh, void* stream);
+int sc_blur_threshold_symmetrize_upper(sc_context* ctx, const float* a, int64_t n, int64_t lda,
+                                       const float* diag_override, double sigma,
+                                       const float* rowmax, double p, double mult, int binarize,
+                                       int preserve_diagonal, int sym_type, float* y, int64_t ldy,
+                                       void* hi, void* lo, int64_t ldh, void* stream);
 
 /* fp32 [n,n] -> split fp16 planes (for matrices that did not come out of the fused pass). */
 int sc_split_planes(sc_context* ctx, const float* a, int64_t n, int64_t lda, void* hi, void* lo,

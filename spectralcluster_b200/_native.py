@@ -51,6 +51,9 @@ PROTOTYPES = {
                              c_ptr],
     "sc_threshold_symmetrize_upper": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_dbl, c_dbl, c_int, c_int,
                                       c_int, c_ptr, c_i64, c_ptr, c_ptr, c_i64, c_ptr],
+    "sc_blur_threshold_symmetrize_upper": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_dbl, c_ptr, c_dbl,
+                                           c_dbl, c_int, c_int, c_int, c_ptr, c_i64, c_ptr, c_ptr,
+                                           c_i64, c_ptr],
     "sc_split_planes": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_i64, c_ptr],
     "sc_diffuse": [c_ptr, c_int, c_int, c_ptr, c_i64, c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_i64,
                    c_ptr, c_ptr, c_ptr],

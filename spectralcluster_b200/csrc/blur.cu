@@ -9,9 +9,11 @@
 //   EPI_STORE materialises B for the generic (unfused) operator API.
 // The blur is recomputed rather than stored: 18 FMAs per element are free next to 4+4 bytes.
 //
-// Whole-matrix, symmetric input (the single-GPU hot path) goes one step further (EPI_UPPER +
-// k_thrsym_upper): B = blur(A) is symmetric, so only the tiles that touch the upper triangle are
-// blurred -- ONCE.  Pass 1 reads half of A, stores that half of B and folds both the row maxima
+// Whole-matrix, symmetric input goes one step further.  The single-GPU hot path (k_blur_pair) blurs
+// only the upper triangle, twice: pass 1 keeps the row and column maxima, pass 2 writes Y and its
+// mirror -- 2 + 2 + 2 B per element of the matrix for the hi plane, no B in memory.  The stored-B
+// form stays for callers that pass a B (EPI_UPPER + k_thrsym_upper): B = blur(A) is symmetric,
+// so only the tiles that touch the upper triangle are blurred -- once.  Pass 1 reads half of A, stores that half of B and folds both the row maxima
 // and the column maxima of every tile into m (m_i = max_j B_ij needs the lower half only through
 // B_ji).  Pass 2 is element-wise on the stored half of B and writes Y(i,j) and Y(j,i) (transposed
 // through shared memory).  HBM traffic 2 + 2 + 2 + 2 = 8 B per element of the matrix when only the
@@ -21,7 +23,8 @@
 //
 // Kernels: k_blur_band<4, EPI> (compile-time radius 4 = sigma ~ 1, the configuration every
 // BASELINE config uses: register sliding windows, cp.async pipeline), k_blur_generic<EPI>
-// (run-time radius <= 64), k_noblur<EPI> (radius 0 and sigma <= 1e-15) and k_thrsym_upper.
+// (run-time radius <= 64), k_noblur<EPI> (radius 0 and sigma <= 1e-15), k_thrsym_upper and
+// k_blur_pair<PASS2> (radius 4).
 #include "common.cuh"
 
 #include <cstdlib>
@@ -668,6 +671,256 @@ k_thrsym_upper(const UpperArgs g) {
   }
 }
 
+// ------------------------------------------------------------------ symmetric pair, blur recomputed
+// The symmetric pair without a stored B: pass 1 (k_blur_pair<false>) folds the row and column maxima
+// of blur(A) over the same elements EPI_UPPER folds -- row i from column 128 floor(i / 128) -- and
+// pass 2 (k_blur_pair<true>) blurs the upper triangle again and writes Y(i, j) and Y(j, i), i <= j,
+// from the one value rule(b[i, j], m_i, m_j).  Each b is the same fmaf chain as k_blur_band's
+// (vertical taps, then horizontal, reflected edges, the crop substituted on read), so m and Y are
+// bit for bit those of sc_blur_upper_rowmax + sc_threshold_symmetrize_upper.
+//
+// A warp owns a strip of 120 output columns and walks down a band of 256 rows with no barrier:
+//   lane L loads the 4 columns c0 - 4 + 4L .. +3 of each input row (one 128-bit load; lanes 0 and 31
+//     are the horizontal halo), PU rows per step with the next step's rows already in flight;
+//   the vertical taps slide down a 16-row register window per column;
+//   the horizontal taps take the 4 columns on each side from the neighbouring lanes (8 shuffles).
+// Halo: 8 rows per 256 (3 %) from HBM; the 8 halo columns of a strip are the next strips' columns and
+// come from L2.  Pass 2 writes Y(i, .) from registers and stages 16 rows of y per warp in shared memory
+// so that Y(j, i0 .. i0 + 15) of the mirror goes out as whole 32-byte sectors of each plane.
+// A CTA is 8 adjacent strips of one band; pass 1 combines their row maxima in shared memory, so there
+// is one atomic per row per CTA and one per column per warp.
+constexpr int PW = 8, PCOLS = 120, PTH = 256, PU = 4, PMB = 16;
+
+struct PairArgs {
+  const float* a;
+  int64_t n, lda;
+  const float* diag;       // optional replacement of a[i][i]
+  float* m_out;            // pass 1: row maxima, zero-filled by the caller
+  int zero_diag;           // pass 1: the diagonal folds as 0 (RowWiseThreshold preserve_diagonal)
+  RuleArgs r;              // pass 2
+};
+
+// One warp's strip: columns [c0, c0 + PCOLS) of rows [r0, r0 + PTH).  FAST: interior and off the
+// diagonal (no reflection, no crop, no per-element masks).
+template <bool PASS2, bool FAST>
+__device__ __forceinline__ void pair_strip(const PairArgs& g, const BlurWeights& bw, int64_t r0,
+                                           int64_t c0, bool vec, float* part, float* ybuf) {
+  constexpr int R = 4;
+  const int lane = threadIdx.x & 31;
+  const int64_t n = g.n;
+  const int64_t cv0 = c0 - R + 4 * lane;                        // this lane's first (virtual) column
+  const bool own = lane >= 1 && lane <= 30;
+  int64_t pc[4];                                                // physical columns (reflected)
+#pragma unroll
+  for (int q = 0; q < 4; ++q) pc[q] = (FAST || vec) ? cv0 + q : reflect_index(cv0 + q, n);
+  const bool crop = !FAST && g.diag != nullptr;
+
+  float cut_j[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+  if (PASS2) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      cut_j[q] = (cv0 + q >= 0 && cv0 + q < n ? g.r.m[cv0 + q] : 0.0f) * g.r.p;
+  }
+  float cm[4] = {0.0f, 0.0f, 0.0f, 0.0f};                       // pass 1: column maxima
+
+  auto load_row = [&](int64_t vr, float (&v)[4]) {
+    const int64_t gr = (FAST || (vr >= 0 && vr < n)) ? vr : reflect_index(vr, n);
+    const float* row = g.a + gr * g.lda;
+    if (FAST || vec) {
+      const float4 t = ld_stream4(row + cv0);
+      v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+    } else {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) v[q] = row[pc[q]];
+    }
+    if (crop) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        if (gr == pc[q]) v[q] = g.diag[gr];
+    }
+  };
+
+  // output row i from the 9 input rows win[.][u .. u + 2R]
+  auto row_out = [&](int64_t i, const float (&win)[4][PU + 2 * R], int u) {
+    float mid[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      float acc = 0.0f;
+#pragma unroll
+      for (int k = 0; k <= 2 * R; ++k) acc = fmaf(bw.w[k], win[q][u + k], acc);
+      mid[q] = acc;
+    }
+    float e[12];                                                // columns cv0 - 4 .. cv0 + 7
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      e[q] = __shfl_up_sync(0xffffffffu, mid[q], 1);
+      e[4 + q] = mid[q];
+      e[8 + q] = __shfl_down_sync(0xffffffffu, mid[q], 1);
+    }
+    float b[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      float acc = 0.0f;
+#pragma unroll
+      for (int k = 0; k <= 2 * R; ++k) acc = fmaf(bw.w[k], e[q + k], acc);
+      b[q] = acc;
+    }
+    const int rl = (int)(i - r0);
+    if (!PASS2) {
+      // fold row i from column 128 floor(i / 128), the diagonal as 0 if asked (EPI_UPPER's set)
+      const int64_t jlo = i & ~(int64_t)127;
+      float v = 0.0f;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int64_t j = cv0 + q;
+        float x = b[q];
+        if (!FAST && g.zero_diag && i == j) x = 0.0f;
+        if (!own || (!FAST && !(i < n && j < n && j >= jlo))) x = 0.0f;
+        x = fmaxf(x, 0.0f);
+        cm[q] = fmaxf(cm[q], x);
+        v = fmaxf(v, x);
+      }
+      // non-negative floats order like their bit patterns: one REDUX.MAX for the strip's row
+      const int mx = __reduce_max_sync(0xffffffffu, __float_as_int(v));
+      if (lane == 0) part[rl] = __int_as_float(mx);
+    } else {
+      const RuleArgs& r = g.r;
+      const float cut_i = r.m[(FAST || i < n) ? i : n - 1] * r.p;
+      float y[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        y[q] = thrsym_rule(r, b[q], cut_i, cut_j[q], !FAST && i == cv0 + q);
+      // Y(i, j) for j >= i
+      if (FAST || (i < n && cv0 >= i && cv0 + 3 < n)) {
+        if (own) store_y<4>(r, i, cv0, y, true, n);
+      } else if (own && i < n) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float yq[1] = {y[q]};
+          if (cv0 + q >= i && cv0 + q < n) store_y<1>(r, i, cv0 + q, yq, true, n);
+        }
+      }
+      *reinterpret_cast<float4*>(ybuf + (rl & (PMB - 1)) * 128 + 4 * lane) =
+          make_float4(y[0], y[1], y[2], y[3]);
+    }
+  };
+
+  // pass 2: Y(j, i0 .. i0 + PMB - 1) <- the staged y(i0 .., j), for the strip's columns j > i
+  auto flush = [&](int64_t i0) {
+    __syncwarp();
+#pragma unroll
+    for (int rd = 0; rd < 4; ++rd) {
+      const int cl = 4 + 32 * rd + lane;                        // column of the staging buffer
+      const int64_t j = c0 + 32 * rd + lane;
+      if (cl >= 4 + PCOLS || (!FAST && j >= n)) continue;
+      float y[PMB];
+#pragma unroll
+      for (int t = 0; t < PMB; ++t) y[t] = ybuf[t * 128 + cl];
+      if (FAST || i0 + PMB - 1 < j) {
+        store_y<PMB>(g.r, j, i0, y, true, n);
+      } else {
+#pragma unroll
+        for (int t = 0; t < PMB; ++t) {
+          const float yt[1] = {y[t]};
+          if (i0 + t < j) store_y<1>(g.r, j, i0 + t, yt, true, n);
+        }
+      }
+    }
+    __syncwarp();
+  };
+
+  // win[q][k] = input row i0 - R + k of the lane's column q, i0 = the step's first output row; the
+  // next step's PU rows are in flight (nxt) while this step is filtered
+  float win[4][PU + 2 * R];
+  float nxt[PU][4];
+#pragma unroll
+  for (int k = 0; k < 2 * R; ++k) {
+    float v[4];
+    load_row(r0 - R + k, v);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) win[q][k] = v[q];
+  }
+#pragma unroll
+  for (int u = 0; u < PU; ++u) load_row(r0 + R + u, nxt[u]);
+  for (int st = 0; st < PTH / PU; ++st) {
+    const int64_t i0 = r0 + (int64_t)st * PU;
+#pragma unroll
+    for (int u = 0; u < PU; ++u)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) win[q][2 * R + u] = nxt[u][q];
+    if (st + 1 < PTH / PU) {
+#pragma unroll
+      for (int u = 0; u < PU; ++u) load_row(i0 + PU + R + u, nxt[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < PU; ++u) row_out(i0 + u, win, u);
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+#pragma unroll
+      for (int k = 0; k < 2 * R; ++k) win[q][k] = win[q][PU + k];
+    if (PASS2 && ((st + 1) * PU) % PMB == 0) flush(i0 + PU - PMB);
+  }
+  if (!PASS2 && own) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+      if (FAST || cv0 + q < n) atomic_max_nonneg(g.m_out + cv0 + q, cm[q]);
+  }
+}
+
+template <bool PASS2>
+__global__ void __launch_bounds__(PW * 32, 2)
+k_blur_pair(const PairArgs g, const BlurWeights bw) {
+  constexpr int R = 4;
+  extern __shared__ float psmem[];     // pass 1: [PW][PTH] row maxima; pass 2: [PW][PMB][128] y
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t n = g.n;
+  const int64_t r0 = (int64_t)blockIdx.x * PTH;
+  // strips from the one holding column r0: every element the band needs lies right of it (PTH is a
+  // multiple of 128)
+  const int64_t s0 = r0 / PCOLS + (int64_t)blockIdx.y * PW;
+  if (s0 * PCOLS >= n) return;                                  // block-uniform
+  const int64_t c0 = (s0 + warp) * PCOLS;
+  float* part = psmem + warp * PTH;
+  float* ybuf = psmem + warp * (PMB * 128);
+  if (c0 < n) {                                                 // warp-uniform
+    const bool vec = c0 >= R && c0 + PCOLS + R <= n && (g.lda & 3) == 0 &&
+                     (reinterpret_cast<uintptr_t>(g.a) & 15) == 0;
+    if (vec && r0 >= R && r0 + PTH + R <= n && c0 >= r0 + PTH + 2 * R)
+      pair_strip<PASS2, true>(g, bw, r0, c0, vec, part, ybuf);
+    else
+      pair_strip<PASS2, false>(g, bw, r0, c0, vec, part, ybuf);
+  } else if (!PASS2) {
+    for (int k = lane; k < PTH; k += 32) part[k] = 0.0f;
+  }
+  if (!PASS2) {
+    __syncthreads();
+    const int rl = threadIdx.x;                                 // PTH == blockDim.x
+    if (r0 + rl < n) {
+      float v = 0.0f;
+#pragma unroll
+      for (int w = 0; w < PW; ++w) v = fmaxf(v, psmem[w * PTH + rl]);
+      atomic_max_nonneg(g.m_out + r0 + rl, v);
+    }
+  }
+}
+
+static_assert(PTH == PW * 32 && PTH % 128 == 0 && PTH % PMB == 0 && PMB % PU == 0,
+              "band geometry");
+
+// Launch one pass of the pair (radius 4 only; the weights come from make_weights).
+template <bool PASS2>
+static int launch_pair(const PairArgs& g, const BlurWeights& bw, cudaStream_t st) {
+  const size_t smem = sizeof(float) * (PASS2 ? PW * PMB * 128 : PW * PTH);
+  auto k = k_blur_pair<PASS2>;
+  SC_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int64_t nstrips = (g.n + PCOLS - 1) / PCOLS;
+  const dim3 grid((unsigned)((g.n + PTH - 1) / PTH), (unsigned)((nstrips + PW - 1) / PW));
+  k<<<grid, PW * 32, smem, st>>>(g, bw);
+  sc::launched();
+  SC_LAUNCH_CHECK();
+  return 0;
+}
+
 // scipy _gaussian_kernel1d: radius = int(truncate * sigma + 0.5) with truncate = 4; sigma <= 1e-15
 // copies the input ("if sigma > 1e-15 ... else output[...] = input[...]"), i.e. radius 0.
 static int blur_radius(double sigma) { return sigma > 1e-15 ? (int)(4.0 * sigma + 0.5) : 0; }
@@ -869,25 +1122,61 @@ extern "C" int sc_blur_threshold_symmetrize_block(
                           binarize, preserve_diagonal, sym_type, y, ldy, hi, lo, ldh, stream);
 }
 
-// ---- symmetric whole-matrix pair (single-GPU hot path).  Pass 1: b_out <- the tiles of blur(a)
-// that touch the upper triangle (the rest of b_out is left untouched), m_out[i] <- max_j blur(a)[i,j]
-// assembled from the row AND column maxima of those tiles.  Requires a symmetric `a` and sigma
+// ---- symmetric whole-matrix pair (single-GPU hot path).  Pass 1: m_out[i] <- max_j blur(a)[i,j]
+// assembled from the row AND column maxima of the tiles of blur(a) that touch the upper triangle;
+// with b_out, those tiles are also stored (the rest of b_out is left untouched) for
+// sc_threshold_symmetrize_upper, without it nothing else is written and
+// sc_blur_threshold_symmetrize_upper blurs the tiles again.  Requires a symmetric `a` and sigma
 // with radius 4 (sigma in [0.875, 1.125), every BASELINE configuration); the caller falls back to
 // sc_gaussian_blur_rowmax + sc_blur_threshold_symmetrize otherwise.
 extern "C" int sc_blur_upper_rowmax(sc_context* ctx, const float* a, int64_t n, int64_t lda,
                                     const float* diag_override, double sigma, int zero_diagonal,
                                     float* b_out, int64_t ldb, float* rowmax_out, void* stream) {
-  SC_REQUIRE(ctx && a && b_out && rowmax_out && n > 0, "sc_blur_upper_rowmax: bad arguments");
+  SC_REQUIRE(ctx && a && rowmax_out && n > 0, "sc_blur_upper_rowmax: bad arguments");
   SC_REQUIRE(blur_radius(sigma) == 4,
              "sc_blur_upper_rowmax: the symmetric pass is built for radius 4 (sigma ~ 1)");
   SC_REQUIRE(n <= 65535LL * 32, "sc_blur_upper_rowmax: n too large for the tile grid");
-  SC_REQUIRE(vec_ok_f32(b_out, ldb), "blur: `out` needs a 16-byte aligned base and ldo %% 4 == 0");
+  SC_REQUIRE(!b_out || vec_ok_f32(b_out, ldb),
+             "blur: `out` needs a 16-byte aligned base and ldo %% 4 == 0");
+  BlurWeights bw;
+  int radius;
+  make_weights(sigma, bw, radius);
+  SC_CUDA(cudaMemsetAsync(rowmax_out, 0, sizeof(float) * n, as_stream(stream)));
+  if (!b_out) {
+    PairArgs p = {};
+    p.a = a; p.n = n; p.lda = lda; p.diag = diag_override;
+    p.m_out = rowmax_out; p.zero_diag = zero_diagonal;
+    return launch_pair<false>(p, bw, as_stream(stream));
+  }
   BlurArgs g = blur_args(a, n, lda, 0, 0, n, diag_override);
   g.out = b_out; g.ldo = ldb; g.rowmax_out = rowmax_out; g.stats_zero_diag = zero_diagonal;
-  BlurWeights bw;
-  make_weights(sigma, bw, g.radius);
-  SC_CUDA(cudaMemsetAsync(rowmax_out, 0, sizeof(float) * n, as_stream(stream)));
+  g.radius = radius;
   return launch_band<EPI_UPPER>(g, bw, as_stream(stream));
+}
+
+// Pass 2 without a stored B: the upper triangle of blur(a) again, then Y(i, j) and Y(j, i) from
+// rule(b[min(i, j), max(i, j)], m_i, m_j) -- bit for bit sc_threshold_symmetrize_upper on the B
+// that sc_blur_upper_rowmax stores.
+extern "C" int sc_blur_threshold_symmetrize_upper(sc_context* ctx, const float* a, int64_t n,
+                                                  int64_t lda, const float* diag_override,
+                                                  double sigma, const float* rowmax, double p,
+                                                  double mult, int binarize, int preserve_diagonal,
+                                                  int sym_type, float* y, int64_t ldy, void* hi,
+                                                  void* lo, int64_t ldh, void* stream) {
+  const char* who = "sc_blur_threshold_symmetrize_upper";
+  SC_REQUIRE(ctx && a && rowmax && n > 0, "%s: bad arguments", who);
+  SC_REQUIRE(blur_radius(sigma) == 4, "%s: the symmetric pass is built for radius 4 (sigma ~ 1)",
+             who);
+  SC_REQUIRE(n <= 65535LL * PCOLS, "%s: n too large for the tile grid", who);
+  PairArgs g = {};
+  if (int rc = rule_args(who, rowmax, p, mult, binarize, preserve_diagonal, sym_type, y, ldy, hi,
+                         lo, ldh, g.r))
+    return rc;
+  g.a = a; g.n = n; g.lda = lda; g.diag = diag_override;
+  BlurWeights bw;
+  int radius;
+  make_weights(sigma, bw, radius);
+  return launch_pair<true>(g, bw, as_stream(stream));
 }
 
 // Pass 2 over the tile pairs (TI, TJ), TI <= TJ, whose rows TI lie in [row_begin, row_end); `b`

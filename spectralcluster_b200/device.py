@@ -146,6 +146,14 @@ def blur_radius(sigma: float) -> int:
   return int(4.0 * sigma + 0.5) if sigma > 1e-15 else 0
 
 
+class DeferredBlur(typing.NamedTuple):
+  """Pass 1 of the symmetric blur pair without a stored B: what pass 2 needs to blur the upper
+  tiles of `a` (with `diag` substituted on read) again."""
+  a: typing.Any
+  diag: typing.Any
+  sigma: float
+
+
 class Engine:
   """One per CUDA device: the sc_context plus allocation / launch helpers."""
 
@@ -235,6 +243,7 @@ class Engine:
       "sc_blur_upper_rowmax": "refinement.GaussianBlur",
       "sc_blur_threshold_symmetrize": "refinement.RowWiseThreshold+Symmetrize",
       "sc_threshold_symmetrize_upper": "refinement.RowWiseThreshold+Symmetrize",
+      "sc_blur_threshold_symmetrize_upper": "refinement.RowWiseThreshold+Symmetrize",
       "sc_row_threshold": "refinement.RowWiseThreshold", "sc_symmetrize": "refinement.Symmetrize",
       "sc_diffuse": "refinement.Diffuse", "sc_gemm_nt_planes": "refinement.Diffuse",
       "sc_row_normalize": "refinement.RowWiseNormalize", "sc_row_stats": "refinement.RowWiseNormalize",
@@ -370,17 +379,21 @@ class Engine:
               0 if hi is None else hi.stride(0), self.stream)
     return y, hi, lo
 
-  def blur_upper_rowmax(self, a, n, sigma, diag, zero_diag):
-    """Symmetric pass 1: (b with its upper tiles = blur(a), m = row maxima of blur(a))."""
+  def blur_upper_rowmax(self, a, n, sigma, diag, zero_diag, store_b=False):
+    """Symmetric pass 1: (b, m = row maxima of blur(a)).  b is a DeferredBlur record, and
+    threshold_symmetrize_upper blurs a's upper tiles again; with store_b it is a matrix whose upper
+    tiles hold blur(a)."""
     t = torch()
-    b = self.matrix(n)
+    b = self.matrix(n) if store_b else None
     m = self.vector(n, t.float32)
     self.call("sc_blur_upper_rowmax", _ptr(a), n, a.stride(0), _ptr(diag), float(sigma),
-              int(bool(zero_diag)), _ptr(b), b.stride(0), _ptr(m), self.stream)
-    return b, m
+              int(bool(zero_diag)), _ptr(b), 0 if b is None else b.stride(0), _ptr(m), self.stream)
+    return (b if store_b else DeferredBlur(a, diag, float(sigma))), m
 
   def threshold_symmetrize_upper(self, b, n, rowmax, p, mult, binarize, preserve_diag, sym_type,
                                  want_f32, want_planes, want_lo=True):
+    """Symmetric pass 2: Y and its mirror from b, a DeferredBlur record (the blur is recomputed)
+    or a matrix holding the upper tiles of blur(a)."""
     t = torch()
     y = self.matrix(n) if want_f32 else None
     hi = lo = None
@@ -388,10 +401,14 @@ class Engine:
       hi, lo = self.planes(n)
     elif want_planes:      # a single-MMA Diffuse reads only the hi plane: 2 B/element less to write
       hi = t.empty((n, round_up(n, 64)), dtype=t.float16, device=self.device)
-    self.call("sc_threshold_symmetrize_upper", _ptr(b), n, b.stride(0), _ptr(rowmax), float(p),
-              float(mult), int(bool(binarize)), int(bool(preserve_diag)), int(sym_type), _ptr(y),
-              0 if y is None else y.stride(0), _ptr(hi), _ptr(lo),
-              0 if hi is None else hi.stride(0), self.stream)
+    rule = (_ptr(rowmax), float(p), float(mult), int(bool(binarize)), int(bool(preserve_diag)),
+            int(sym_type), _ptr(y), 0 if y is None else y.stride(0), _ptr(hi), _ptr(lo),
+            0 if hi is None else hi.stride(0), self.stream)
+    if isinstance(b, DeferredBlur):
+      self.call("sc_blur_threshold_symmetrize_upper", _ptr(b.a), n, b.a.stride(0), _ptr(b.diag),
+                b.sigma, *rule)
+    else:
+      self.call("sc_threshold_symmetrize_upper", _ptr(b), n, b.stride(0), *rule)
     return y, hi, lo
 
   @staticmethod
@@ -970,7 +987,8 @@ def run_refinement(eng: Engine, a, n: int, options, crop_vector=None, a_symmetri
       sym_type = (nat.SYMMETRIZE_MAX if options.symmetrize_type == rf.SymmetrizeType.Max
                   else nat.SYMMETRIZE_AVERAGE)
       if eng.upper_pass_ok(sigma):
-        # blur(A) is symmetric: blur the upper tiles once, keep them, mirror the result
+        # blur(A) is symmetric: pass 1 keeps only the row maxima of its upper tiles, pass 2 blurs
+        # them again and writes Y and its mirror
         b, m = eng.blur_upper_rowmax(cur, n, sigma, diag, zero_diag)
         want_lo = (diffuse_precision if diffuse_precision is not None
                    else eng.gemm_precision) != nat.GEMM_SINGLE
