@@ -157,6 +157,7 @@ class SpectralClusterer:
     n_vectors = min(n, max(limit, self.min_clusters or 0))
     op = (refined.s, n, delta, left, right, sign)
     counted = None          # (k, gap) when the solver already ran the eigengap
+    fallback = None         # why a Lanczos solve gave way to the dense solver
     top = None              # lambda_max when w is a prefix of an ascending spectrum
     if not refined.symmetric:
       # not symmetric nor diagonally similar to a symmetric matrix (e.g. RowWiseThreshold without
@@ -182,9 +183,19 @@ class SpectralClusterer:
       top_solve = lambda: eng.eigh_factored(*fop, nat.EIG_LARGEST, 1, 0)[0]
     elif n > eng.dense_eig_max and lanczos_fits(n, limit):
       solver = "lanczos"
-      w, v, stats = eng.eigh(*op, which, limit, n_vectors, False)
-      stats = stats.tolist()
-      top_solve = lambda: eng.eigh(*op, nat.EIG_LARGEST, 1, 0, False)[0]
+      try:
+        w, v, stats = eng.eigh(*op, which, limit, n_vectors, False)
+        stats = stats.tolist()
+        top_solve = lambda: eng.eigh(*op, nat.EIG_LARGEST, 1, 0, False)[0]
+      except nat.NativeError as e:
+        # a wanted pair did not converge within the product budget: the values next to it crowd
+        # within tol * lambda_max (as the nonzero Laplacian values of the near-complete components
+        # Diffuse leaves do).  The dense solver takes any stored S up to DENSE_MAX_N, as on the
+        # dense route below.
+        if n > DENSE_MAX_N or "eigenpairs converged" not in str(e):
+          raise
+        solver, stats, top_solve, fallback = "dense", None, None, str(e)
+        w, v, _ = eng.eigh(*op, which, n, n_vectors, True)
     elif n > DENSE_MAX_N or refined.y_hi is not None:
       # more pairs than one Lanczos solve finds, above the dense solver's n: windows of block
       # Lanczos on the complement of the pairs found, until the eigengap is decided; on the
@@ -225,6 +236,8 @@ class SpectralClusterer:
     k, gap = counted or self._count_clusters(w, descend, top)
     self.last_details = dict(eigenvalues=np.array(w[:limit]), n_clusters_raw=k, max_gap=gap,
                              solver=solver, lanczos_stats=stats)
+    if fallback is not None:
+      self.last_details["lanczos_fallback"] = fallback
     if refined.tiles is not None:
       computed, total = refined.tiles.tolist()
       self.last_details["diffuse"] = dict(tiles=computed, of=total, operator="factored")

@@ -246,3 +246,18 @@ def test_dense_limit_mirrors_the_native_guard():
   src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))),
                           "spectralcluster_b200", "csrc", "eigh_dense.cu")).read()
   assert "SC_REQUIRE(n <= %d," % scb.spectral_clusterer.DENSE_MAX_N in src
+
+
+def lanczos_block_size(n_values):
+  """sc_eigh_block_size restated: vectors per block for n_values pairs."""
+  return 4 if n_values <= 4 else 8 if n_values <= 8 else 12 if n_values <= 12 else 16
+
+
+@pytest.mark.parametrize("limit", range(1, scb.spectral_clusterer.LANCZOS_MAX_PAIRS + 1))
+def test_lanczos_fits_implies_the_native_basis_requirement(limit):
+  """Whenever predict() picks one Lanczos solve (lanczos_fits), sc_eigh_extremal takes it: with
+  b = sc_eigh_block_size(limit) it needs n >= 2 * 7 * b (six processed blocks and the one in
+  flight, twice)."""
+  fits = [n for n in range(1, 2048) if scb.spectral_clusterer.lanczos_fits(n, limit)]
+  assert fits and fits == list(range(fits[0], 2048))           # monotone in n
+  assert fits[0] >= 2 * 7 * lanczos_block_size(limit)

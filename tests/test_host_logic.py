@@ -240,3 +240,44 @@ def test_eigen_stage_solver_choice(monkeypatch, case, calls, solver):
   limit = n if not max_clusters else min(n, max_clusters + 1)
   assert len(sc.last_details["eigenvalues"]) == min(limit, len(w))
   assert (sc.last_details["lanczos_stats"] is None) == (solver == "dense")
+
+
+class StallingEngine(FakeEngine):
+  """A FakeEngine whose Lanczos solves of more than one pair stop short of convergence."""
+
+  def __init__(self, n, message="sc_eigh_extremal: only 7 of 26 eigenpairs converged to 1e-09 in "
+               "20000 matrix-vector products"):
+    super().__init__(n)
+    self.message = message
+
+  def eigh(self, s, n, delta, left, right, sign, which, n_values, n_vectors, dense, tol=1e-9,
+           max_matvecs=0):
+    if not dense and n_values > 1:
+      self._rec("eigh", which, n_values, n_vectors, dense)
+      raise nat.NativeError(self.message)
+    return super().eigh(s, n, delta, left, right, sign, which, n_values, n_vectors, dense)
+
+
+@pytest.mark.parametrize("eigengap", [RATIO, NDIFF])
+def test_unconverged_lanczos_falls_back_to_the_dense_solver(eigengap):
+  """A stored S whose Lanczos solve does not converge is solved by the dense solver, as on the
+  dense route (the whole spectrum, so no lambda_max solve), and last_details says why."""
+  eng = StallingEngine(2000)
+  sc = scb.SpectralClusterer(max_clusters=25, laplacian_type=UNNORM, eigengap_type=eigengap)
+  w, v, k, gap = sc._eigen_on_device(eng, scb.spectral_clusterer.DeviceAffinity("A", 2000))
+  solves = [c for c in eng.calls if c[0] != "row_stats"]
+  assert solves == [("eigh", S, 26, 26, False), ("eigh", S, 2000, 26, True)]
+  assert sc.last_details["solver"] == "dense" and sc.last_details["lanczos_stats"] is None
+  assert "eigenpairs converged" in sc.last_details["lanczos_fallback"]
+  assert len(sc.last_details["eigenvalues"]) == 26 and k == 3 and v == "V"
+
+
+def test_other_lanczos_errors_and_large_n_still_raise():
+  """Only non-convergence falls back, and only where the dense solver takes n."""
+  sc = scb.SpectralClusterer(max_clusters=25, laplacian_type=UNNORM)
+  eng = StallingEngine(2000, message="sc_eigh_extremal: bad arguments")
+  with pytest.raises(nat.NativeError, match="bad arguments"):
+    sc._eigen_on_device(eng, scb.spectral_clusterer.DeviceAffinity("A", 2000))
+  n = scb.spectral_clusterer.DENSE_MAX_N + 1
+  with pytest.raises(nat.NativeError, match="eigenpairs converged"):
+    sc._eigen_on_device(StallingEngine(n), scb.spectral_clusterer.DeviceAffinity("A", n))
