@@ -611,6 +611,19 @@ int sc_cluster_centroids(sc_context* ctx, const void* x, int x_is_f64, int64_t n
 int sc_average_linkage(sc_context* ctx, double* dist, int64_t n, int64_t ldd, int64_t* merge_xy,
                        double* merge_dist, int64_t* merge_size, void* stream);
 
+/* ---- NN-chain of a small matrix in one thread block -----------------------------------------
+ * The matrices of MultiStageClusterer's steps (at most U2 = 600 rows by default) are too small for
+ * the grid barriers of sc_complete_linkage / sc_average_linkage to pay off.  sc_nn_chain_small runs
+ * the same chain in one thread block, with block barriers: for linkage SC_LINKAGE_COMPLETE it
+ * returns exactly what sc_complete_linkage returns on the same dist, for SC_LINKAGE_AVERAGE exactly
+ * what sc_average_linkage returns (same merges in the same chain order, same distances and sizes,
+ * bit for bit), with the same arguments and contract otherwise.  2 <= n <= SC_NN_SMALL_MAX; a chain
+ * top without a neighbour below infinity (non-finite dist) is an error.  SYNCHRONOUS. */
+enum { SC_LINKAGE_COMPLETE = 0, SC_LINKAGE_AVERAGE = 1 };
+enum { SC_NN_SMALL_MAX = 2048 };   /* the measured crossing: DESIGN.md §5 */
+int sc_nn_chain_small(sc_context* ctx, double* dist, int64_t n, int64_t ldd, int linkage,
+                      int64_t* merge_xy, double* merge_dist, int64_t* merge_size, void* stream);
+
 /* ---- fallback_clusterer.check_single_cluster, AffinityGmmBic (fallback_clusterer.py:158-178) --
  * scikit-learn's GaussianMixture(1) and (2) fitted to affinity[np.triu_indices(n, offset)], as
  * one streaming reduction per step; the KMeans / EM / BIC control flow is host logic

@@ -146,6 +146,7 @@ PROTOTYPES = {
                              c_ptr],
     "sc_complete_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_average_linkage": [c_ptr, c_ptr, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr],
+    "sc_nn_chain_small": [c_ptr, c_ptr, c_i64, c_i64, c_int, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_gmm_band_pass": [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_int, c_ptr, c_ptr, c_ptr, c_ptr],
     "sc_gmm_band_pass_packed": [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_int, c_ptr, c_ptr, c_ptr,
                                 c_ptr],
@@ -163,6 +164,8 @@ GEMM_SPLIT3, GEMM_SINGLE, GEMM_SPLIT2 = 0, 1, 2
 ABI_VERSION = 2
 EIG_LARGEST, EIG_SMALLEST = 0, 1
 DTYPE_F32, DTYPE_F64, DTYPE_F16, DTYPE_BF16 = 0, 1, 2, 3
+LINKAGE_COMPLETE, LINKAGE_AVERAGE = 0, 1
+NN_SMALL_MAX = 2048           # SC_NN_SMALL_MAX: the largest n sc_nn_chain_small takes
 
 _lib = None
 _lock = threading.Lock()

@@ -8,6 +8,8 @@
 //                      a row scan split across the grid (one CTA per SM), a grid barrier, and a
 //                      redundant reduction of the per-CTA minima in every CTA; a merge adds a
 //                      row + column update (the linkage's Lance-Williams rule) and one more barrier.
+//   k_nn_chain_small<L> the same chain for n <= SC_NN_SMALL_MAX in one CTA: block barriers instead
+//                      of grid barriers, sizes and chain in shared memory (stream-sized caches)
 // and the centroids of the clusters found (utils.get_cluster_centroids, max_spectral_size):
 //   k_centroid_order   stable counting sort of the row indices by cluster id, one warp
 //   k_centroid_sums    per (cluster, column): fp64 sum of the members in row order, over the count
@@ -133,7 +135,31 @@ __device__ __forceinline__ void warp_min_idx(double& v, int& i) {
   }
 }
 
+// The (value, index) minimum of a CTA's NN_THREADS pairs: each warp reduces its lanes, lane 0
+// stages the warp's pair, and warp 0 reduces the staged pairs.  The result is valid in warp 0.
+__device__ __forceinline__ void cta_min_idx(double& v, int& i, double* red_v, int* red_i) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  warp_min_idx(v, i);
+  if (lane == 0) red_v[wid] = v, red_i[wid] = i;
+  __syncthreads();
+  if (wid == 0) {
+    v = lane < NN_THREADS / 32 ? red_v[lane] : INFINITY;
+    i = lane < NN_THREADS / 32 ? red_i[lane] : INT_MAX;
+    warp_min_idx(v, i);
+  }
+}
+
 enum class Linkage { Complete, Average };
+
+// The Lance-Williams update of d(i, a u b) from d(i, a), d(i, b) and the sizes na, nb, nab = na + nb.
+// Average is scipy's _average, (na d_ai + nb d_bi) / (na + nb), rounded step by step: a contracted
+// FMA would round once less and break bitwise equality with scipy.
+template <Linkage L>
+__device__ __forceinline__ double merged_distance(double da, double db, double na, double nb,
+                                                  double nab) {
+  if constexpr (L == Linkage::Complete) return fmax(da, db);
+  else return __ddiv_rn(__dadd_rn(__dmul_rn(na, da), __dmul_rn(nb, db)), nab);
+}
 
 // Every CTA runs the same chain bookkeeping on the same reduced values, so all agree on every
 // decision without a broadcast.  D and size change inside the launch: they are read with
@@ -264,6 +290,95 @@ __global__ void k_fill_ones(int* p, int64_t n) {
   if (i < n) p[i] = 1;
 }
 
+// k_nn_chain's chain, scan order, tie rules and updates in one CTA, for the small matrices of a
+// stream, where k_nn_chain's grid barriers cost more than the scans.  Every thread keeps the same
+// chain bookkeeping; sizes and the chain live in shared memory (2 n ints), and D is read and
+// written with plain loads and stores, which __syncthreads orders within the CTA.  Every branch
+// below depends only on values all threads share (k, len, x, prev, y), so every thread reaches
+// every barrier, up to the last merge.  *status is 1 if a chain top had no neighbour below
+// infinity (non-finite D), 0 otherwise.
+template <Linkage L>
+__global__ void __launch_bounds__(NN_THREADS)
+k_nn_chain_small(double* dist, int n, int64_t ldd, int64_t* __restrict__ m_xy,
+                 double* __restrict__ m_dist, int64_t* __restrict__ m_size,
+                 int* __restrict__ status) {
+  extern __shared__ int ns_smem[];
+  int* size = ns_smem;          // [n]
+  int* chain = ns_smem + n;     // [n]
+  __shared__ double red_v[NN_THREADS / 32];
+  __shared__ int red_i[NN_THREADS / 32];
+  __shared__ double s_min;
+  __shared__ int s_y;
+  for (int i = threadIdx.x; i < n; i += NN_THREADS) size[i] = 1;
+  if (threadIdx.x == 0) *status = 0;
+  __syncthreads();
+  int len = 0, x = -1, prev = -1, lo = 0;
+  for (int k = 0; k < n - 1;) {
+    if (len == 0) {
+      while (size[lo] == 0) ++lo;
+      x = lo, prev = -1, len = 1;
+      if (threadIdx.x == 0) chain[0] = x;
+    }
+    // a merge in this step joins x and prev: their sizes, read before thread 0 rewrites them
+    const int nx = size[x], nprev = prev >= 0 ? size[prev] : 0;
+    const double* row = dist + (int64_t)x * ldd;
+    double bv = INFINITY;
+    int bi = INT_MAX;
+    for (int i = threadIdx.x; i < n; i += NN_THREADS) {
+      if (i == x || size[i] == 0) continue;
+      const double v = row[i];
+      if (v < bv) bv = v, bi = i;
+    }
+    cta_min_idx(bv, bi, red_v, red_i);
+    if (threadIdx.x == 0) {
+      if (prev >= 0) {                         // the previous chain element wins a tie
+        const double dp = row[prev];
+        if (dp <= bv) bv = dp, bi = prev;
+      }
+      s_min = bv, s_y = bi;
+    }
+    // the next writes of s_y / s_min and of the staged pairs follow the next step's first barrier,
+    // which every thread reaches only after reading them here
+    __syncthreads();
+    const int y = s_y;
+    const double dmin = s_min;
+    if (y == INT_MAX) {
+      if (threadIdx.x == 0) *status = 1;
+      return;
+    }
+    if (y != prev) {                           // grow the chain
+      if (threadIdx.x == 0) chain[len] = y;
+      ++len, prev = x, x = y;
+      continue;
+    }
+    // ---- merge x and y into max(x, y); retire min(x, y)
+    const int a = x < y ? x : y, b = x < y ? y : x;
+    const double* ra = dist + (int64_t)a * ldd;
+    double* rb = dist + (int64_t)b * ldd;
+    const double na = a == x ? nx : nprev, nb = a == x ? nprev : nx, nab = nx + nprev;
+#pragma unroll 1
+    for (int i = threadIdx.x; i < n; i += NN_THREADS) {
+      if (i == a || i == b || size[i] == 0) continue;
+      const double v = merged_distance<L>(ra[i], rb[i], na, nb, nab);
+      rb[i] = v;
+      dist[i * ldd + b] = v;
+    }
+    if (threadIdx.x == 0) {                    // no thread reads size[a] or size[b] in this phase
+      const int sz = size[a] + size[b];
+      m_xy[2 * k] = a, m_xy[2 * k + 1] = b, m_dist[k] = dmin, m_size[k] = sz;
+      size[b] = sz;
+      size[a] = 0;
+    }
+    __syncthreads();
+    ++k;
+    len -= 2;
+    if (len > 0) {
+      x = chain[len - 1];
+      prev = len > 1 ? chain[len - 2] : -1;
+    }
+  }
+}
+
 }  // namespace
 
 extern "C" int sc_cosine_distances_f64(sc_context* ctx, const void* x, int x_is_f64, int64_t n,
@@ -346,6 +461,41 @@ extern "C" int sc_average_linkage(sc_context* ctx, double* dist, int64_t n, int6
                                   void* stream) {
   return nn_chain_linkage<Linkage::Average>("sc_average_linkage", ctx, dist, n, ldd, merge_xy,
                                             merge_dist, merge_size, stream);
+}
+
+extern "C" int sc_nn_chain_small(sc_context* ctx, double* dist, int64_t n, int64_t ldd, int linkage,
+                                 int64_t* merge_xy, double* merge_dist, int64_t* merge_size,
+                                 void* stream) {
+  SC_REQUIRE(ctx && dist && merge_xy && merge_dist && merge_size && n >= 2 && ldd >= n &&
+             (linkage == SC_LINKAGE_COMPLETE || linkage == SC_LINKAGE_AVERAGE),
+             "sc_nn_chain_small: bad arguments");
+  SC_REQUIRE(n <= SC_NN_SMALL_MAX, "sc_nn_chain_small: n = %lld is above SC_NN_SMALL_MAX = %d",
+             (long long)n, (int)SC_NN_SMALL_MAX);
+  cudaStream_t st = as_stream(stream);
+  const int64_t m = n - 1;
+  // one scratch: xy [2m] int64 | size [m] int64 | distance [m] fp64 | status int
+  Scratch out;
+  SC_CUDA(out.alloc(sizeof(int64_t) * 4 * m + sizeof(int), st));
+  int64_t* xy = out.as<int64_t>();
+  int64_t* ms = xy + 2 * m;
+  double* md = reinterpret_cast<double*>(ms + m);
+  int* status = reinterpret_cast<int*>(md + m);
+  static_assert(sizeof(int) * 2 * SC_NN_SMALL_MAX <= 48 * 1024,
+                "sizes and chain fit the default dynamic shared memory");
+  const size_t smem = sizeof(int) * 2 * n;
+  auto kernel = linkage == SC_LINKAGE_COMPLETE ? k_nn_chain_small<Linkage::Complete>
+                                               : k_nn_chain_small<Linkage::Average>;
+  kernel<<<1, NN_THREADS, smem, st>>>(dist, (int)n, ldd, xy, md, ms, status);
+  SC_LAUNCH_CHECK();
+  launched(1);
+  int bad = 0;
+  SC_CUDA(cudaMemcpyAsync(merge_xy, xy, sizeof(int64_t) * 2 * m, cudaMemcpyDeviceToHost, st));
+  SC_CUDA(cudaMemcpyAsync(merge_dist, md, sizeof(double) * m, cudaMemcpyDeviceToHost, st));
+  SC_CUDA(cudaMemcpyAsync(merge_size, ms, sizeof(int64_t) * m, cudaMemcpyDeviceToHost, st));
+  SC_CUDA(cudaMemcpyAsync(&bad, status, sizeof(int), cudaMemcpyDeviceToHost, st));
+  SC_CUDA(cudaStreamSynchronize(st));
+  SC_REQUIRE(!bad, "sc_nn_chain_small: a chain top has no nearest neighbour (non-finite distances)");
+  return 0;
 }
 
 // ---- utils.get_cluster_centroids: np.add.at into fp64 sums, then division by np.bincount ----------

@@ -64,6 +64,15 @@ def bounded_tile_count(n: int) -> int:
              for m in range(-(-n // LIST_BM)))
 
 
+def nn_chain_entry(linkage: int, n: int) -> str:
+  """The NN-chain kernel for n rows, chosen by n alone: one thread block up to nat.NN_SMALL_MAX
+  (DESIGN.md §5 has the measured crossing), the cooperative grid above."""
+  if n <= nat.NN_SMALL_MAX:
+    return "sc_nn_chain_small"
+  return {nat.LINKAGE_COMPLETE: "sc_complete_linkage",
+          nat.LINKAGE_AVERAGE: "sc_average_linkage"}[linkage]
+
+
 def panel_rows_for(n: int) -> int:
   """Rows per panel of the factored route: about FACTORED_PANEL_BYTES of fp32 rows, a multiple of
   PANEL_ALIGN, chosen from n alone."""
@@ -268,6 +277,7 @@ class Engine:
       "sc_cosine_distances_f64": "AgglomerativeClustering(cosine)",
       "sc_complete_linkage": "AgglomerativeClustering(cosine, complete)",
       "sc_average_linkage": "AgglomerativeClustering(cosine, average)",
+      "sc_nn_chain_small": "AgglomerativeClustering(cosine)",
       "sc_naive_cluster": "naive_clusterer.NaiveClusterer",
   }
   nvtx = os.environ.get("SCB_NVTX") == "1"
@@ -752,12 +762,12 @@ class Engine:
   def complete_linkage(self, dist, n: int):
     """Complete-linkage NN-chain over the device distance matrix (overwritten) -> host
     (xy int64 [n-1, 2], distance fp64 [n-1], size int64 [n-1]), in chain order."""
-    return self._nn_chain("sc_complete_linkage", dist, n)
+    return self.nn_chain(nn_chain_entry(nat.LINKAGE_COMPLETE, n), dist, n, nat.LINKAGE_COMPLETE)
 
   def average_linkage(self, dist, n: int):
     """Average-linkage NN-chain over the device distance matrix (overwritten) -> host
     (xy int64 [n-1, 2], distance fp64 [n-1], size int64 [n-1]), in chain order."""
-    return self._nn_chain("sc_average_linkage", dist, n)
+    return self.nn_chain(nn_chain_entry(nat.LINKAGE_AVERAGE, n), dist, n, nat.LINKAGE_AVERAGE)
 
   def naive_cluster(self, x_dev, threshold: float, adaptation_threshold: float, stop_at: int = 0,
                     means=None, counts=None):
@@ -785,11 +795,14 @@ class Engine:
     k = clusters.value
     return labels[:processed.value], processed.value, k, m[:k], c[:k]
 
-  def _nn_chain(self, entry, dist, n: int):
+  def nn_chain(self, entry: str, dist, n: int, linkage: int):
+    """The NN-chain entry `entry` (one of nn_chain_entry's answers) for an nat.LINKAGE_* linkage;
+    complete_linkage / average_linkage choose the entry by n."""
     xy = np.empty((n - 1, 2), dtype=np.int64)
     md = np.empty(n - 1, dtype=np.float64)
     ms = np.empty(n - 1, dtype=np.int64)
-    self.call(entry, _ptr(dist), n, dist.stride(0), xy.ctypes.data_as(ctypes.c_void_p),
+    head = (_ptr(dist), n, dist.stride(0)) + ((linkage,) if entry == "sc_nn_chain_small" else ())
+    self.call(entry, *head, xy.ctypes.data_as(ctypes.c_void_p),
               md.ctypes.data_as(ctypes.c_void_p), ms.ctypes.data_as(ctypes.c_void_p), self.stream)
     return xy, md, ms
 

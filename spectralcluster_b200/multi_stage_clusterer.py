@@ -7,7 +7,9 @@ embeddings, beyond that an agglomerative pre-clusterer compresses the cache to U
 the spectral clusterer (device path) labels; the cache itself is replaced by its centroids every
 time it reaches U2.  Host logic around `SpectralClusterer.predict` exactly as in the reference; the
 complete-linkage cosine pre-clusterer runs on the device with scikit-learn's labels
-(agglomerative.py).
+(agglomerative.py).  A stream of CUDA tensors keeps its cache on the device (torch.cat for
+np.vstack, device centroids at a compression) and returns what the stream of their host twins
+returns; labels stay host arrays.
 """
 
 from __future__ import annotations
@@ -17,7 +19,9 @@ import enum
 import numpy as np
 
 from . import agglomerative
+from . import device as dev
 from . import fallback_clusterer
+from . import naive_clusterer
 from . import utils
 
 
@@ -46,6 +50,20 @@ def match_labels(current: np.ndarray, previous: np.ndarray) -> np.ndarray:
   return table[current]
 
 
+def twin_dtype(x):
+  """The numpy dtype of a tensor's host twin (x.cpu().numpy(); bfloat16 through float32)."""
+  t = dev.torch()
+  return np.dtype(np.float32) if x.dtype == t.bfloat16 else t.empty(0, dtype=x.dtype).numpy().dtype
+
+
+def append_rows(cache, embedding):
+  """np.vstack([cache, embedding]) for tensors: the rows of both, in the dtype np.vstack gives
+  their host twins."""
+  t = dev.torch()
+  dtype = t.from_numpy(np.empty(0, np.result_type(twin_dtype(cache), twin_dtype(embedding)))).dtype
+  return t.cat([t.atleast_2d(cache).to(dtype), t.atleast_2d(embedding.detach()).to(dtype)])
+
+
 class MultiStageClusterer:
   """multi_stage_clusterer.py:67-180."""
 
@@ -67,15 +85,38 @@ class MultiStageClusterer:
     self.num_embeddings = 0
     self.compression_labels = None       # original embedding -> row of the cache
     self.previous_output = None
+    self.stream_device = None            # the device of a stream of CUDA tensors
 
-  def streaming_predict(self, embedding: np.ndarray) -> np.ndarray:
-    """Labels of every embedding seen so far, earlier ones possibly corrected."""
+  def streaming_predict(self, embedding) -> np.ndarray:
+    """Labels of every embedding seen so far, earlier ones possibly corrected.
+
+    `embedding` is one row, (d,) or (1, d): an ndarray, or a CUDA tensor on the current device.
+    A stream of CUDA tensors returns, step for step, what the stream of their host twins returns
+    (X.cpu().numpy(); bfloat16: X.float().cpu().numpy()).  A stream that mixes host arrays and
+    CUDA tensors, or CUDA tensors of two devices, raises TypeError, and the step changes nothing."""
+    device = embedding.device if naive_clusterer._is_cuda_tensor(embedding) else None
+    if self.num_embeddings and device != self.stream_device:
+      raise TypeError("this stream takes %s, got %s" % (
+          "host arrays" if self.stream_device is None else "CUDA tensors on %s" % self.stream_device,
+          "a host array" if device is None else "a CUDA tensor on %s" % device))
+    if device is not None and device.index != dev.torch().cuda.current_device():
+      raise ValueError("the embedding is on %s, but streaming_predict() runs on cuda:%d (the "
+                       "current device)" % (device, dev.torch().cuda.current_device()))
     self.num_embeddings += 1
     if self.num_embeddings == 1:
+      self.stream_device = device
+      # the first embedding is the cache as given (1-D stays 1-D); bfloat16 as its twin, float32
       self.cache = embedding
+      if device is not None:
+        self.cache = embedding.detach()
+        if self.cache.dtype == dev.torch().bfloat16:
+          self.cache = self.cache.float()
       self.previous_output = np.array([0])
       return self.previous_output
-    self.cache = np.vstack([self.cache, embedding])
+    if device is None:
+      self.cache = np.vstack([self.cache, embedding])
+    else:
+      self.cache = append_rows(self.cache, embedding)
     if self.num_embeddings <= self.U1:                        # fallback or main clusterer alone
       self.previous_output = self.main.predict(self.cache)
       return self.previous_output

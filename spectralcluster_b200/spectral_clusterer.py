@@ -338,11 +338,7 @@ class SpectralClusterer:
     on_device = not isinstance(embeddings, np.ndarray)
     x = dev.twin(embeddings) if on_device else embeddings
     pre = agglomerative.CosineCompleteLinkage(n_clusters=self.max_spectral_size).fit_predict(x)
-    if on_device:
-      centroids = dev.Engine.get().cluster_centroids(x, pre)
-    else:
-      centroids = utils.get_cluster_centroids(embeddings, pre)
-    return utils.chain_labels(pre, self.predict(centroids))
+    return utils.chain_labels(pre, self.predict(utils.get_cluster_centroids(x, pre)))
 
   # ------------------------------------------------------------------ predict
   def predict(self, embeddings, constraint_matrix=None) -> np.ndarray:

@@ -12,6 +12,7 @@ import numpy as np
 
 from . import _native as nat
 from . import device as dev
+from . import naive_clusterer
 
 EPS = 1e-10
 
@@ -110,8 +111,14 @@ def enforce_ordered_labels(labels: np.ndarray) -> np.ndarray:
   return out
 
 
-def get_cluster_centroids(embeddings: np.ndarray, labels: np.ndarray) -> np.ndarray:
-  """Mean embedding of every cluster 0..max(labels) (utils.py:159-177), as one segmented sum."""
+def get_cluster_centroids(embeddings, labels: np.ndarray):
+  """Mean embedding of every cluster 0..max(labels) (utils.py:159-177), as one segmented sum.
+
+  A CUDA tensor gives a device fp64 tensor (sc_cluster_centroids) whose host copy equals what the
+  host function returns for the tensor's host twin, bit for bit."""
+  if naive_clusterer._is_cuda_tensor(embeddings):
+    x = dev.twin(dev.device_embeddings(embeddings))
+    return dev.Engine.get(x.device.index).cluster_centroids(x, labels)
   labels = np.asarray(labels).astype(np.int64)
   k = int(labels.max()) + 1
   sums = np.zeros((k, embeddings.shape[1]), dtype=np.result_type(embeddings.dtype, np.float64))
